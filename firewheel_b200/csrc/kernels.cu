@@ -725,10 +725,6 @@ __global__ void __launch_bounds__(128) sampler_kernel(const __grid_constant__ Sa
 // K-resampler: polyphase windowed-sinc sample player (SURVEY §8 a13, spec in include/fw_b200.h). One thread = one output
 // frame of one (voice, channel): the read position is analytic (pos + n * step, Q32.32), so frames are independent.
 // Accumulation order (taps ascending, separate multiply and add) matches the oracle bit for bit.
-__global__ void resampler_begin_kernel(uint64_t* pos, const uint64_t* seek, uint32_t* seek_flag, uint32_t V) {
-    const uint32_t v = blockIdx.x * blockDim.x + threadIdx.x;
-    if (v < V && seek_flag[v]) { pos[v] = seek[v] << 32; seek_flag[v] = 0; }
-}
 __global__ void resampler_end_kernel(uint64_t* pos, const uint64_t* step, const uint32_t* flags, const uint32_t* res, uint32_t V, uint32_t frames) {
     const uint32_t v = blockIdx.x * blockDim.x + threadIdx.x;
     if (v < V && (flags[v] & 1u) && res[v] != 0) pos[v] += (uint64_t)frames * step[v];
@@ -919,10 +915,6 @@ cudaError_t launch_sampler(const SamplerArgs& a, cudaStream_t st) {
     const bool vec4 = (a.frames % 4 == 0) && (a.block_frames % 4 == 0) && (al % 16 == 0) && (a.out_vstride % 4 == 0);
     if (vec4) return launch_pdl(sampler_kernel<4>, dim3(a.num_voices, (a.frames / 4 + 127) / 128, a.n_out), dim3(128), st, a);
     return launch_pdl(sampler_kernel<1>, dim3(a.num_voices, (a.frames + 127) / 128, a.n_out), dim3(128), st, a);
-}
-cudaError_t launch_resampler_begin(uint64_t* pos, const uint64_t* seek, uint32_t* seek_flag, uint32_t V, cudaStream_t st) {
-    resampler_begin_kernel<<<(V + 127) / 128, 128, 0, st>>>(pos, seek, seek_flag, V);
-    return cudaGetLastError();
 }
 cudaError_t launch_resampler(const ResamplerArgs& a, uint64_t* pos, cudaStream_t st) {
     if (a.n_out && a.num_voices && a.frames) {

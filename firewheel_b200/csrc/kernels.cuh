@@ -14,7 +14,6 @@ cudaError_t launch_control(const ControlArgs& a, cudaStream_t st);
 cudaError_t launch_chain(const ChainArgs& a, bool bus, cudaStream_t st);
 uint32_t chain_voice_groups(uint32_t num_voices);  // partial buses produced by the bus variant
 cudaError_t launch_sum(const SumArgs& a, cudaStream_t st);
-cudaError_t launch_resampler_begin(uint64_t* pos, const uint64_t* seek, uint32_t* seek_flag, uint32_t V, cudaStream_t st);
 cudaError_t launch_resampler(const ResamplerArgs& a, uint64_t* pos, cudaStream_t st);  // data kernel + position advance
 cudaError_t launch_sampler(const SamplerArgs& a, cudaStream_t st);
 cudaError_t launch_silence_fix(const SilenceFixArgs& a, cudaStream_t st);

@@ -245,9 +245,8 @@ struct NodeDeviceState {
         return ok;
     }
     // at call start: pin the resource table a resampler reads during this call
-    bool snapshot_params(cudaStream_t) {
+    void snapshot_params() {
         if (kind == FW_NODE_RESAMPLER) res_table->snapshot(&cur_tab, &cur_n_res);
-        return true;
     }
 };
 
@@ -257,9 +256,11 @@ struct Plan {
     std::vector<std::shared_ptr<NodeDeviceState>> states;   // keeps every referenced node state alive
     std::vector<Id> nodes_to_remove;
     CtlTables tables{}; uint64_t* d_flags = nullptr;
-    // data plane: stages run in order; pointwise stages are fused chain programs, temporal stages own state
-    struct Stage { int kind = 0; /* 0 pointwise, 1 temporal */ ChainProgram prog{}; uint32_t c_in = 0, c_out = 0;
-                   std::shared_ptr<NodeDeviceState> biquad, delay, reverb, sampler, svf; int sampler_sm = -1; };  // kind 2: reverb, kind 3: sampler head
+    // data plane: stages run in order; pointwise stages are fused chain programs, the others own state
+    enum StageKind { STAGE_POINTWISE, STAGE_TEMPORAL, STAGE_REVERB, STAGE_SAMPLER };  // STAGE_SAMPLER: a SamplerNode heading the chain
+    // node: the biquad or SVF of a temporal stage (none: a lone delay), the reverb, the sampler; delay: a temporal stage's delay line
+    struct Stage { StageKind kind = STAGE_POINTWISE; ChainProgram prog{}; uint32_t c_in = 0, c_out = 0;
+                   std::shared_ptr<NodeDeviceState> node, delay; int sampler_sm = -1; };
     std::vector<Stage> stages;
     // generic lowering (arbitrary DAG of built-in nodes): one launch group per scheduled node over pool buffers [buffer][V][T]
     struct GNode { uint32_t kind = 0; std::vector<uint32_t> in_buf, out_buf; std::vector<uint8_t> in_clear; int sm0 = -1, sm1 = -1, mask_slot = -1, custom_idx = -1, sampler_idx = -1;
@@ -390,6 +391,9 @@ struct ProfScope {  // brackets the launches of one kernel class with a pair of 
     }
     ~ProfScope() { if (on) { cudaEventRecord(p->prof_ev[p->prof_used + 1], p->stream); p->prof_used += 2; } }
 };
+// One launch of `n` kernels inside a profile scope of class `cls` (0 control, 1 chain / pointwise, 2 combine, 3 temporal / reverb /
+// resampler): false on a CUDA error, else the kernels are counted.
+#define FW_LAUNCH(p, cls, n, call) ([&]() -> bool { ProfScope ps_((p), (cls)); if (!FW_CUDA(call)) return false; (p)->launches += (n); return true; }())
 
 // =============================================================================================
 // lowering: schedule -> control tables + fused chain program
@@ -462,22 +466,21 @@ static bool lower(fw_ctx* c, const Schedule& s, Plan* plan, std::string* why) {
     size_t first = 1;
     if (width == 0 && n >= 3 && tb.nodes[1].kind == FW_NODE_SAMPLER && s.nodes[1].in.empty() && s.nodes[1].out.size() >= 1 && s.nodes[1].out.size() <= 2) {
         // no stream inputs: a SamplerNode heads the chain (BASELINE config 5: sampler -> gain -> pan -> ... -> bus)
-        Plan::Stage hs; hs.kind = 3; hs.c_in = 0; hs.c_out = (uint32_t)s.nodes[1].out.size(); hs.sampler = c->node_states[s.nodes[1].id.pack()]; hs.sampler_sm = sm_of_node[1];
+        Plan::Stage hs; hs.kind = Plan::STAGE_SAMPLER; hs.c_in = 0; hs.c_out = (uint32_t)s.nodes[1].out.size(); hs.node = c->node_states[s.nodes[1].id.pack()]; hs.sampler_sm = sm_of_node[1];
         plan->stages.push_back(hs);
         width = hs.c_out; prev = s.nodes[1].id; first = 2;
     }
     if (width < 1 || width > 2) { *why = "the fused chain supports 1 or 2 channels"; return false; }
-    plan->c_in = (uint32_t)gin.out.size();
     auto fed_by_prev = [&](const SchedNode& sn, uint32_t w) {
         if (sn.in.size() != w) return false;
         for (uint32_t p = 0; p < w; ++p) if (sn.in[p].should_clear || sn.in[p].producer != prev || sn.in[p].producer_port != p) return false;
         return true;
     };
-    Plan::Stage cur; cur.kind = 0; cur.prog.c_in = width; cur.c_in = width;
+    Plan::Stage cur; cur.prog.c_in = width; cur.c_in = width;
     bool cur_open = true;  // a pointwise stage is being accumulated
     auto close_pointwise = [&](bool force) {
         if (cur_open && (cur.prog.n_ops > 0 || force)) { cur.prog.c_out = width; cur.c_out = width; plan->stages.push_back(cur); }
-        cur = Plan::Stage{}; cur.kind = 0; cur.prog.c_in = width; cur.c_in = width; cur_open = true;
+        cur = Plan::Stage{}; cur.prog.c_in = width; cur.c_in = width; cur_open = true;
     };
     for (size_t i = first; i + 1 < n; ++i) {
         const SchedNode& sn = s.nodes[i];
@@ -487,14 +490,14 @@ static bool lower(fw_ctx* c, const Schedule& s, Plan* plan, std::string* why) {
         const uint32_t kind = nr->params->kind;
         if (kind == FW_NODE_CONV_REVERB) {
             close_pointwise(false);
-            Plan::Stage ts; ts.kind = 2; ts.c_in = ts.c_out = width; ts.reverb = c->node_states[sn.id.pack()];
+            Plan::Stage ts; ts.kind = Plan::STAGE_REVERB; ts.c_in = ts.c_out = width; ts.node = c->node_states[sn.id.pack()];
             plan->stages.push_back(ts);
             prev = sn.id;
             continue;
         }
         if (kind == FW_NODE_SVF) {
             close_pointwise(false);
-            Plan::Stage ts; ts.kind = 1; ts.c_in = ts.c_out = width; ts.svf = c->node_states[sn.id.pack()];
+            Plan::Stage ts; ts.kind = Plan::STAGE_TEMPORAL; ts.c_in = ts.c_out = width; ts.node = c->node_states[sn.id.pack()];
             plan->stages.push_back(ts);
             prev = sn.id;
             continue;
@@ -502,13 +505,13 @@ static bool lower(fw_ctx* c, const Schedule& s, Plan* plan, std::string* why) {
         if (kind == FW_NODE_BIQUAD || kind == FW_NODE_DELAY) {
             std::shared_ptr<NodeDeviceState> st = c->node_states[sn.id.pack()];
             // a delay directly after a biquad joins its pass; anything else opens a new temporal stage
-            if (kind == FW_NODE_DELAY && !plan->stages.empty() && plan->stages.back().kind == 1 && !plan->stages.back().delay &&
-                plan->stages.back().biquad && cur.prog.n_ops == 0) {
+            if (kind == FW_NODE_DELAY && !plan->stages.empty() && plan->stages.back().kind == Plan::STAGE_TEMPORAL && !plan->stages.back().delay &&
+                plan->stages.back().node && plan->stages.back().node->kind == FW_NODE_BIQUAD && cur.prog.n_ops == 0) {
                 plan->stages.back().delay = st;
             } else {
                 close_pointwise(false);
-                Plan::Stage ts; ts.kind = 1; ts.c_in = ts.c_out = width;
-                if (kind == FW_NODE_BIQUAD) ts.biquad = st; else ts.delay = st;
+                Plan::Stage ts; ts.kind = Plan::STAGE_TEMPORAL; ts.c_in = ts.c_out = width;
+                if (kind == FW_NODE_BIQUAD) ts.node = st; else ts.delay = st;
                 plan->stages.push_back(ts);
             }
             prev = sn.id;
@@ -534,7 +537,7 @@ static bool lower(fw_ctx* c, const Schedule& s, Plan* plan, std::string* why) {
     if (!fed_by_prev(gout, width)) { *why = "graph_out is not fed port-to-port by the end of the chain"; return false; }
     // the last stage must be pointwise when the master bus follows it, and a plan is never empty
     const bool bus = c->cfg.master_bus != 0;
-    close_pointwise(plan->stages.empty() || (bus && cur.prog.n_ops == 0 && plan->stages.back().kind != 0));
+    close_pointwise(plan->stages.empty() || (bus && cur.prog.n_ops == 0 && plan->stages.back().kind != Plan::STAGE_POINTWISE));
     plan->c_out = width;
     return true;
     };  // chain_lower
@@ -1398,8 +1401,7 @@ static int run_bus_stage(fw_processor* p, Plan& pl, ChainArgs& xa, uint32_t n_ou
     }
     if (n == 1) { xa.out = bus_dst; xa.bus_pitch = bus_pitch; }
     else { xa.out = pl.d_part[0]; xa.bus_pitch = 0; }
-    { ProfScope ps(p, 1); if (!FW_CUDA(launch_chain(xa, true, p->stream))) return FW_PROC_DEVICE_ERROR; }
-    p->launches++;
+    if (!FW_LAUNCH(p, 1, 1, launch_chain(xa, true, p->stream))) return FW_PROC_DEVICE_ERROR;
     // With several ranks and the exchange on the side stream, the kernel that completes the rank-local bus also publishes the exchange
     // epoch (last CTA done -> device word): the main stream then has exactly the kernels of the single-GPU case.
     const bool in_line = pl.heavy_stage;
@@ -1440,62 +1442,128 @@ static int run_bus_stage(fw_processor* p, Plan& pl, ChainArgs& xa, uint32_t n_ou
     return FW_PROC_OK;
 }
 
+// ---- launches of the stateful node kinds, shared by the fused-chain stages (enqueue_chunk) and the generic lowering --------------
+// C channels of every voice: row v * C + k (voice v, channel k) starts at in + row * in_pitch and at out + row * out_pitch floats.
+// A fused-chain stage passes all its channels as one block ([V][C][pitch]); the generic lowering passes every channel as a block
+// of its own (C = 1): a pool buffer [V][T] or, as input, one channel of the caller's rows (in_pitch = n_in * Tfull).
+struct RowBlock { const float* in; float* out; uint32_t C; uint64_t in_pitch, out_pitch; };
+static uint32_t channels_of(const RowBlock* b, uint32_t nb) { uint32_t n = 0; for (uint32_t i = 0; i < nb; ++i) n += b[i].C; return n; }
+
+// SamplerNode: one launch writes the output rows of every block.
+static int run_sampler(fw_processor* p, const Plan& pl, const NodeDeviceState& st, const SmpRec* srec, int sm, const RowBlock* b, uint32_t nb, uint32_t T) {
+    SamplerArgs sa{};
+    for (uint32_t i = 0; i < nb; ++i) {
+        for (uint32_t k = 0; k < b[i].C; ++k) sa.out[sa.n_out++] = b[i].out + k * b[i].out_pitch;
+        sa.out_vstride = b[i].C * b[i].out_pitch;
+    }
+    sa.num_voices = p->num_voices; sa.frames = T; sa.block_frames = pl.block_frames;
+    sa.srec = srec; sa.res = st.d_res; sa.loop_start = st.d_loop_start; sa.res_tab = st.cur_tab; sa.sm = sm; sa.rec = pl.rec;
+    return FW_LAUNCH(p, 1, 1, launch_sampler(sa, p->stream)) ? FW_PROC_OK : FW_PROC_DEVICE_ERROR;
+}
+
+// Biquad or SVF cascade (`filter`) and / or delay line. Two one-channel blocks share a pass as its two row segments: twice the rows
+// per launch. The state / ring row of voice v, channel c is v * nc + c; blocks of all nc channels or of one get there with
+// srow_mul = nc / C. Every pass of a chunk starts at the same ring cursor, which then advances once.
+static int run_temporal(fw_processor* p, const NodeDeviceState* filter, NodeDeviceState* delay, const RowBlock* b, uint32_t nb, uint32_t T, uint32_t zero_first) {
+    const uint32_t V = p->num_voices, nc = channels_of(b, nb), D = delay ? delay->params->delay : 0u;
+    for (uint32_t i = 0, c = 0; i < nb; i += 2) {
+        const uint32_t segs = i + 1 < nb ? 2u : 1u;
+        TemporalArgs ta{};
+        ta.in = b[i].in; ta.out = b[i].out; ta.in_pitch = (uint32_t)b[i].in_pitch; ta.out_pitch = (uint32_t)b[i].out_pitch;
+        ta.R = segs * V * b[i].C; ta.C = b[i].C; ta.T = T; ta.zero_first = zero_first; ta.srow_mul = nc / b[i].C; ta.srow_add = c;
+        if (segs == 2) { ta.in2 = b[i + 1].in; ta.out2 = b[i + 1].out; ta.seg_rows = V * b[i].C; }
+        if (filter) { ta.svf = filter->kind == FW_NODE_SVF ? 1u : 0u; ta.ns = filter->params->num_stages; ta.coeffs = filter->d_coeffs; ta.state = filter->d_state; }
+        if (D) { ta.D = D; ta.ring = delay->d_ring; ta.pos = delay->ring_pos; }
+        if (!FW_LAUNCH(p, 3, 1, launch_temporal(ta, p->stream))) return FW_PROC_DEVICE_ERROR;
+        c += segs * b[i].C;
+    }
+    if (D) delay->ring_pos = (uint32_t)(((uint64_t)delay->ring_pos + T) % D);
+    return FW_PROC_OK;
+}
+
+// ConvReverb: one history + GEMM launch per block; history rows of channel c are c * V .. c * V + V - 1. The history cursor
+// advances once per chunk, the GEMM's fix-up epoch once per launch.
+static int run_reverb(fw_processor* p, NodeDeviceState& rs, const RowBlock* b, uint32_t nb, uint32_t T, uint32_t zero_first) {
+    if (T > NodeDeviceState::kReverbMaxFrames) { g_dev_err = "conv reverb: more than 65536 frames in one chunk"; return FW_PROC_BAD_ARGS; }
+    const uint32_t V = p->num_voices, H = reverb_hist(rs.params->ir_len);
+    if (rs.xh_cursor + T > rs.xh_pitch || (rs.xh_cursor & 7u)) {  // buffer full (or cursor off the 16-byte TMA grid after an odd-length call):
+        // carry the H most recent samples to the front of the other buffer
+        if (!FW_CUDA(cudaMemcpy2DAsync(rs.d_xh[rs.xh_cur ^ 1u], (size_t)rs.xh_pitch * 2, static_cast<const uint16_t*>(rs.d_xh[rs.xh_cur]) + (rs.xh_cursor - H),
+                                       (size_t)rs.xh_pitch * 2, (size_t)H * 2, (size_t)V * channels_of(b, nb), cudaMemcpyDeviceToDevice, p->stream))) return FW_PROC_DEVICE_ERROR;
+        rs.xh_cur ^= 1u; rs.xh_cursor = H;
+    }
+    for (uint32_t i = 0, c = 0; i < nb; c += b[i].C, ++i) {
+        ReverbCall rc{};
+        rc.in = b[i].in; rc.out = b[i].out; rc.in_pitch = (uint32_t)b[i].in_pitch; rc.out_pitch = (uint32_t)b[i].out_pitch; rc.xh = rs.d_xh[rs.xh_cur]; rc.bt = rs.d_bt;
+        rc.V = V; rc.C = b[i].C; rc.T = T; rc.L = rs.params->ir_len; rc.ir_ch = rs.params->ir_channels; rc.cursor = rs.xh_cursor; rc.pitch = rs.xh_pitch;
+        rc.zero_first = zero_first; rc.chan_base = c;
+        rc.ws = rs.d_rv_ws; rc.flags = rs.d_rv_flags; rc.epoch = ++rs.rv_epoch;
+        std::string rerr;
+        if (!FW_LAUNCH(p, 3, 2, launch_reverb(rc, p->stream, &rerr))) { if (!rerr.empty()) g_dev_err = rerr; return FW_PROC_DEVICE_ERROR; }
+    }
+    rs.xh_cursor += T;
+    return FW_PROC_OK;
+}
+
 // Generic lowering at run time: walk the scheduled nodes (compiler.rs order) over the pool [buffer][V][Tc]. Buffer reuse
 // is the reference's (compiler.rs:302-412): it is valid for any execution that respects the schedule order, and each
 // node here finishes all blocks of the chunk before the next node starts.
 static int enqueue_generic(fw_processor* p, Plan& pl, const float* d_in, float* d_out, const Chunk& ck) {
     const uint32_t V = p->num_voices, n_in = pl.c_in, n_out = pl.c_out, T = ck.Tc;
     const size_t BS = (size_t)V * T;  // floats per pool buffer
+    const uint64_t in_vs = (uint64_t)n_in * ck.Tfull, out_vs = (uint64_t)n_out * ck.Tfull;  // voice strides of the caller's rows
     auto buf = [&](uint32_t b) { return pl.d_pool + (size_t)b * BS; };
-    if (pl.reads_caller_rows && (uint64_t)n_in * ck.Tfull > 0xffffffffull) { g_dev_err = "input rows of more than 2^32 / channels frames"; return FW_PROC_BAD_ARGS; }
-    // one pointwise launch: up to 2 channels, arbitrary channel pointers
-    auto pointwise = [&](const ChainProgram& prog, const float* i0, const float* i1, uint64_t ivs, float* o0, float* o1, uint64_t ovs, bool first) -> bool {
+    auto caller_in = [&](size_t c) { return d_in + ck.t0 + c * (size_t)ck.Tfull; };
+    if (pl.reads_caller_rows && in_vs > 0xffffffffull) { g_dev_err = "input rows of more than 2^32 / channels frames"; return FW_PROC_BAD_ARGS; }
+    // the inputs of one pointwise launch: up to 2 channels, arbitrary channel pointers; `first`: the caller's rows, not a preceding kernel's output
+    auto chain_args = [&](const ChainProgram& prog, const float* i0, const float* i1, uint64_t ivs, bool first) {
         ChainArgs xa{};
-        xa.in_ch[0] = i0; xa.in_ch[1] = i1 ? i1 : i0; xa.out_ch[0] = o0; xa.out_ch[1] = o1 ? o1 : o0;
-        xa.in_vstride = ivs; xa.out_vstride = ovs; xa.out = nullptr;
+        xa.in_ch[0] = i0; xa.in_ch[1] = i1 ? i1 : i0; xa.in_vstride = ivs;
         xa.num_voices = V; xa.frames = T; xa.block_frames = pl.block_frames; xa.zero_first_block = (first && ck.zero_first) ? 1u : 0u;
         xa.rec = pl.rec; xa.prog = prog; xa.in_from_prev_kernel = first ? 0u : 1u;
-        ProfScope ps(p, 1);
-        if (!FW_CUDA(launch_chain(xa, false, p->stream))) return false;
-        p->launches++;
-        return true;
+        return xa;
+    };
+    auto pointwise = [&](ChainArgs xa, float* o0, float* o1, uint64_t ovs) -> bool {
+        xa.out_ch[0] = o0; xa.out_ch[1] = o1 ? o1 : o0; xa.out_vstride = ovs;
+        return FW_LAUNCH(p, 1, 1, launch_chain(xa, false, p->stream));
     };
     auto prog1 = [&](int kind, uint32_t ci, uint32_t co, int sm0, int sm1, float f0) {
         ChainProgram pr{}; pr.c_in = ci; pr.c_out = co; pr.n_ops = kind < 0 ? 0u : 1u;
         if (kind >= 0) { pr.ops[0].kind = (uint32_t)kind; pr.ops[0].sm0 = sm0; pr.ops[0].sm1 = sm1; pr.ops[0].f0 = f0; }
         return pr;
     };
-    // channel-wise op over matching in/out channel lists, two channels per launch
-    auto per_channel = [&](const Plan::GNode& gn, int kind) -> bool {
-        const size_t nc = std::min(gn.in_buf.size(), gn.out_buf.size());
+    // the node's op `kind` (< 0: copy) over nc one-channel blocks, two channels per launch
+    auto per_channel = [&](const Plan::GNode& gn, int kind, const RowBlock* b, size_t nc, bool first) -> bool {
         for (size_t c = 0; c < nc; c += 2) {
             const bool two = c + 1 < nc;
-            if (!pointwise(prog1(kind, two ? 2 : 1, two ? 2 : 1, gn.sm0, gn.sm1, gn.f0), buf(gn.in_buf[c]), two ? buf(gn.in_buf[c + 1]) : nullptr, T,
-                           buf(gn.out_buf[c]), two ? buf(gn.out_buf[c + 1]) : nullptr, T, false)) return false;
+            const ChainArgs xa = chain_args(prog1(kind, two ? 2 : 1, two ? 2 : 1, gn.sm0, gn.sm1, gn.f0), b[c].in, two ? b[c + 1].in : nullptr, b[c].in_pitch, first);
+            if (!pointwise(xa, b[c].out, two ? b[c + 1].out : nullptr, b[c].out_pitch)) return false;
         }
         return true;
+    };
+    RowBlock rows[64];
+    // the node's first n channels as one-channel blocks: inputs from pool buffers or, fed by graph_in, the caller's rows; outputs to pool buffers
+    auto node_rows = [&](const Plan::GNode& gn, size_t n) -> const RowBlock* {
+        const bool caller = !gn.src_port.empty();
+        for (size_t c = 0; c < n; ++c)
+            rows[c] = RowBlock{c >= gn.in_buf.size() ? nullptr : caller ? caller_in(gn.src_port[c]) : buf(gn.in_buf[c]), buf(gn.out_buf[c]), 1, caller ? in_vs : T, T};
+        return rows;
     };
     auto silence_fix = [&](const Plan::GNode& gn, size_t out_ch, uint64_t test) -> bool {
         if (gn.mask_slot < 0) return true;
         SilenceFixArgs fa{};
         fa.out = buf(gn.out_buf[out_ch]); fa.test = test; fa.num_voices = V; fa.frames = T; fa.block_frames = pl.block_frames; fa.mask_slot = gn.mask_slot; fa.rec = pl.rec;
-        ProfScope ps(p, 1);
-        if (!FW_CUDA(launch_silence_fix(fa, p->stream))) return false;
-        p->launches++;
-        return true;
+        return FW_LAUNCH(p, 1, 1, launch_silence_fix(fa, p->stream));
     };
-    // a (fused) stereo program: the run's ops + `own` (kind < 0: none), from the run's first inputs — pool buffers, or the caller's input
-    // channels when the run head is fed by graph_in — to o0 / o1
-    auto stereo_run = [&](const Plan::GNode& gn, int own_kind, float* o0, float* o1, uint64_t ovs) -> bool {
+    // a fused run: the ops of its absorbed nodes + `own` (kind < 0: none), read from the run's first inputs — pool buffers, or the
+    // caller's input channels when the run head is fed by graph_in
+    auto fused_run = [&](const Plan::GNode& gn, int own_kind) {
         ChainProgram pr{}; pr.c_in = 2; pr.c_out = 2;
         for (const ChainOp& op : gn.pre_ops) pr.ops[pr.n_ops++] = op;
         if (own_kind >= 0) { ChainOp& op = pr.ops[pr.n_ops++]; op = ChainOp{}; op.kind = (uint32_t)own_kind; op.sm0 = gn.sm0; op.sm1 = own_kind == OP_PAN ? gn.sm1 : -1; op.f0 = gn.f0; }
-        if (!gn.src_port.empty()) {
-            const float* base = d_in + ck.t0;
-            return pointwise(pr, base + (size_t)gn.src_port[0] * ck.Tfull, base + (size_t)gn.src_port[1] * ck.Tfull, (uint64_t)n_in * ck.Tfull, o0, o1, ovs, true);
-        }
+        if (!gn.src_port.empty()) return chain_args(pr, caller_in(gn.src_port[0]), caller_in(gn.src_port[1]), in_vs, true);
         const std::vector<uint32_t>& ib = gn.run_in.empty() ? gn.in_buf : gn.run_in;
-        return pointwise(pr, buf(ib[0]), buf(ib[1]), T, o0, o1, ovs, false);
+        return chain_args(pr, buf(ib[0]), buf(ib[1]), T, false);
     };
     const size_t N = pl.gnodes.size();
     for (size_t i = 0; i < N; ++i) {
@@ -1504,87 +1572,63 @@ static int enqueue_generic(fw_processor* p, Plan& pl, const float* d_in, float* 
         for (size_t k = 0; k < gn.in_buf.size(); ++k)  // unconnected inputs are cleared every block (schedule.rs:310-313)
             if (gn.in_clear[k]) { if (!FW_CUDA(launch_fill(buf(gn.in_buf[k]), BS, 0.0f, p->stream))) return FW_PROC_DEVICE_ERROR; p->launches++; }
         if (i == 0) {  // graph_in: stream channels -> pool (prepare_graph_inputs, schedule.rs:213-253)
-            for (size_t c = 0; pl.gin_copy && c < gn.out_buf.size(); c += 2) {
-                const bool two = c + 1 < gn.out_buf.size();
-                const float* s0 = d_in + c * (size_t)ck.Tfull + ck.t0;
-                if (!pointwise(prog1(-1, two ? 2 : 1, two ? 2 : 1, -1, -1, 0.f), s0, two ? s0 + ck.Tfull : nullptr, (uint64_t)n_in * ck.Tfull,
-                               buf(gn.out_buf[c]), two ? buf(gn.out_buf[c + 1]) : nullptr, T, true)) return FW_PROC_DEVICE_ERROR;
-            }
+            if (!pl.gin_copy) continue;
+            for (size_t c = 0; c < gn.out_buf.size(); ++c) rows[c] = RowBlock{caller_in(c), buf(gn.out_buf[c]), 1, in_vs, T};
+            if (!per_channel(gn, -1, rows, gn.out_buf.size(), true)) return FW_PROC_DEVICE_ERROR;
             continue;
         }
         if (i + 1 == N) {  // graph_out: pool -> stream channels / master bus (read_graph_outputs, schedule.rs:255-287)
-            if (pl.bus) {
-                ChainArgs xa{};
-                xa.in_ch[0] = buf(gn.in_buf[0]); xa.in_ch[1] = buf(gn.in_buf[n_out > 1 ? 1 : 0]); xa.in_vstride = T;
-                xa.num_voices = V; xa.frames = T; xa.block_frames = pl.block_frames; xa.rec = pl.rec; xa.prog = prog1(-1, n_out, n_out, -1, -1, 0.f); xa.in_from_prev_kernel = 1;
-                if (!gn.pre_ops.empty()) {  // the pointwise run that ends here rides in the bus stage's program
-                    xa.prog = ChainProgram{}; xa.prog.c_in = 2; xa.prog.c_out = 2;
-                    for (const ChainOp& op : gn.pre_ops) xa.prog.ops[xa.prog.n_ops++] = op;
-                    if (!gn.src_port.empty()) {
-                        const float* base = d_in + ck.t0;
-                        xa.in_ch[0] = base + (size_t)gn.src_port[0] * ck.Tfull; xa.in_ch[1] = base + (size_t)gn.src_port[1] * ck.Tfull; xa.in_vstride = (uint64_t)n_in * ck.Tfull;
-                        xa.in_from_prev_kernel = 0; xa.zero_first_block = ck.zero_first ? 1u : 0u;
-                    } else { xa.in_ch[0] = buf(gn.run_in[0]); xa.in_ch[1] = buf(gn.run_in[1]); }
-                }
+            if (pl.bus) {  // the pointwise run that ends here, if any, rides in the bus stage's program
+                ChainArgs xa = gn.pre_ops.empty() ? chain_args(prog1(-1, n_out, n_out, -1, -1, 0.f), buf(gn.in_buf[0]), buf(gn.in_buf[n_out > 1 ? 1 : 0]), T, false)
+                                                  : fused_run(gn, -1);
                 const int brc = run_bus_stage(p, pl, xa, n_out, ck, d_out + ck.t0);
                 if (brc != FW_PROC_OK) return brc;
             } else if (!gn.pre_ops.empty()) {
                 float* o0 = d_out + ck.t0;
-                if (!stereo_run(gn, -1, o0, o0 + ck.Tfull, (uint64_t)n_out * ck.Tfull)) return FW_PROC_DEVICE_ERROR;
+                if (!pointwise(fused_run(gn, -1), o0, o0 + ck.Tfull, out_vs)) return FW_PROC_DEVICE_ERROR;
             } else {
-                for (size_t c = 0; c < gn.in_buf.size(); c += 2) {
-                    const bool two = c + 1 < gn.in_buf.size();
-                    float* o0 = d_out + c * (size_t)ck.Tfull + ck.t0;
-                    if (!pointwise(prog1(-1, two ? 2 : 1, two ? 2 : 1, -1, -1, 0.f), buf(gn.in_buf[c]), two ? buf(gn.in_buf[c + 1]) : nullptr, T,
-                                   o0, two ? o0 + ck.Tfull : nullptr, (uint64_t)n_out * ck.Tfull, false)) return FW_PROC_DEVICE_ERROR;
-                }
+                for (size_t c = 0; c < gn.in_buf.size(); ++c) rows[c] = RowBlock{buf(gn.in_buf[c]), d_out + ck.t0 + c * (size_t)ck.Tfull, 1, T, out_vs};
+                if (!per_channel(gn, -1, rows, gn.in_buf.size(), false)) return FW_PROC_DEVICE_ERROR;
             }
             continue;
         }
+        const uint32_t zf = gn.src_port.empty() ? 0u : ck.zero_first;  // Q11 applies to the caller's rows only
+        const size_t n_io = std::min(gn.in_buf.size(), gn.out_buf.size());  // channels of a channel-wise op
+        int rc = FW_PROC_OK;
         switch (gn.kind) {
             case FW_NODE_DUMMY: break;  // no outputs (rejected otherwise)
-            case FW_NODE_SAMPLER: {
-                NodeDeviceState& st = *gn.st;
-                SamplerArgs sa{};
-                for (size_t c = 0; c < gn.out_buf.size(); ++c) sa.out[c] = buf(gn.out_buf[c]);
-                sa.out_vstride = T; sa.n_out = (uint32_t)gn.out_buf.size(); sa.num_voices = V; sa.frames = T; sa.block_frames = pl.block_frames;
-                sa.srec = pl.d_srec[gn.sampler_idx]; sa.res = st.d_res; sa.loop_start = st.d_loop_start; sa.res_tab = st.cur_tab; sa.sm = gn.sm0; sa.rec = pl.rec;
-                ProfScope ps(p, 1);
-                if (!FW_CUDA(launch_sampler(sa, p->stream))) return FW_PROC_DEVICE_ERROR;
-                p->launches++;
+            case FW_NODE_SAMPLER:
+                rc = run_sampler(p, pl, *gn.st, pl.d_srec[gn.sampler_idx], gn.sm0, node_rows(gn, gn.out_buf.size()), (uint32_t)gn.out_buf.size(), T);
                 break;
-            }
             case FW_NODE_VOLUME: case FW_NODE_HARD_CLIP:
                 if (gn.kind == FW_NODE_VOLUME && (!gn.pre_ops.empty() || !gn.src_port.empty())) {  // stereo Volume ending a fused run / reading the caller's rows
-                    if (!stereo_run(gn, OP_GAIN, buf(gn.out_buf[0]), buf(gn.out_buf[1]), T)) return FW_PROC_DEVICE_ERROR;
+                    if (!pointwise(fused_run(gn, OP_GAIN), buf(gn.out_buf[0]), buf(gn.out_buf[1]), T)) return FW_PROC_DEVICE_ERROR;
                     break;
                 }
-                if (!per_channel(gn, gn.kind == FW_NODE_VOLUME ? OP_GAIN : OP_CLIP)) return FW_PROC_DEVICE_ERROR;
+                if (!per_channel(gn, gn.kind == FW_NODE_VOLUME ? OP_GAIN : OP_CLIP, node_rows(gn, n_io), n_io, false)) return FW_PROC_DEVICE_ERROR;
                 for (size_t c = 0; gn.mask_slot >= 0 && c < gn.out_buf.size(); ++c) if (!silence_fix(gn, c, 1ull << c)) return FW_PROC_DEVICE_ERROR;
                 break;
             case FW_NODE_PAN:
-                if (!stereo_run(gn, OP_PAN, buf(gn.out_buf[0]), buf(gn.out_buf[1]), T)) return FW_PROC_DEVICE_ERROR;
+                if (!pointwise(fused_run(gn, OP_PAN), buf(gn.out_buf[0]), buf(gn.out_buf[1]), T)) return FW_PROC_DEVICE_ERROR;
                 break;
             case FW_NODE_MONO_TO_STEREO:
-                if (!pointwise(prog1(OP_M2S, 1, 2, -1, -1, 0.f), buf(gn.in_buf[0]), nullptr, T, buf(gn.out_buf[0]), buf(gn.out_buf[1]), T, false)) return FW_PROC_DEVICE_ERROR;
+                if (!pointwise(chain_args(prog1(OP_M2S, 1, 2, -1, -1, 0.f), buf(gn.in_buf[0]), nullptr, T, false), buf(gn.out_buf[0]), buf(gn.out_buf[1]), T)) return FW_PROC_DEVICE_ERROR;
                 if (!silence_fix(gn, 0, 1ull) || !silence_fix(gn, 1, 1ull)) return FW_PROC_DEVICE_ERROR;
                 break;
             case FW_NODE_STEREO_TO_MONO:
-                if (!pointwise(prog1(OP_S2M, 2, 1, -1, -1, 0.f), buf(gn.in_buf[0]), buf(gn.in_buf[1]), T, buf(gn.out_buf[0]), nullptr, T, false)) return FW_PROC_DEVICE_ERROR;
+                if (!pointwise(chain_args(prog1(OP_S2M, 2, 1, -1, -1, 0.f), buf(gn.in_buf[0]), buf(gn.in_buf[1]), T, false), buf(gn.out_buf[0]), nullptr, T)) return FW_PROC_DEVICE_ERROR;
                 if (!silence_fix(gn, 0, 3ull)) return FW_PROC_DEVICE_ERROR;
                 break;
             case FW_NODE_SUM: {
                 const size_t no = gn.out_buf.size(), ports = no ? gn.in_buf.size() / no : 0;
-                if (ports <= 1) { if (!per_channel(gn, -1)) return FW_PROC_DEVICE_ERROR; break; }  // copy (sum.rs:58-65)
+                if (ports <= 1) { if (!per_channel(gn, -1, node_rows(gn, n_io), n_io, false)) return FW_PROC_DEVICE_ERROR; break; }  // copy (sum.rs:58-65)
                 for (size_t c = 0; c < no; ++c) {
                     SumArgs sa{};
                     for (size_t q = 0; q < ports; ++q) { sa.in[q] = buf(gn.in_buf[q * no + c]); sa.mask_bit[q] = (uint8_t)(q * no + c); }
                     sa.out = buf(gn.out_buf[c]); sa.n_ports = (uint32_t)ports; sa.num_voices = V; sa.frames = T; sa.block_frames = pl.block_frames;
                     sa.mask_slot = gn.mask_slot; sa.skip_silent = ports >= 5 ? 1u : 0u;
                     sa.all_mask = gn.in_buf.size() >= 64 ? ~0ull : (1ull << gn.in_buf.size()) - 1ull; sa.rec = pl.rec;
-                    ProfScope ps(p, 1);
-                    if (!FW_CUDA(launch_sum(sa, p->stream))) return FW_PROC_DEVICE_ERROR;
-                    p->launches++;
+                    if (!FW_LAUNCH(p, 1, 1, launch_sum(sa, p->stream))) return FW_PROC_DEVICE_ERROR;
                 }
                 break;
             }
@@ -1596,56 +1640,17 @@ static int enqueue_generic(fw_processor* p, Plan& pl, const float* d_in, float* 
                 uint32_t lg = 0; while ((1u << lg) < st.params->rs_phases) ++lg;
                 ra.phase_shift = 32 - lg;
                 ra.table = st.d_rs_table; ra.pos = st.d_rs_pos; ra.step = st.d_rs_step; ra.flags = st.d_rs_flags; ra.res = st.d_rs_res; ra.res_tab = st.cur_tab;
-                ProfScope ps(p, 3);
-                if (!FW_CUDA(launch_resampler(ra, st.d_rs_pos, p->stream))) return FW_PROC_DEVICE_ERROR;
-                p->launches += 2;
+                if (!FW_LAUNCH(p, 3, 2, launch_resampler(ra, st.d_rs_pos, p->stream))) return FW_PROC_DEVICE_ERROR;
                 break;
             }
-            case FW_NODE_SVF: case FW_NODE_BIQUAD: case FW_NODE_DELAY: {  // two channels (two pool buffers) per pass: twice the rows per launch
-                NodeDeviceState& st = *gn.st;
-                const uint32_t nc = (uint32_t)gn.in_buf.size(), D = gn.kind == FW_NODE_DELAY ? st.params->delay : 0u;
-                for (uint32_t c = 0; c < nc; c += 2) {
-                    const bool two = c + 1 < nc;
-                    TemporalArgs ta{};
-                    ta.in = buf(gn.in_buf[c]); ta.out = buf(gn.out_buf[c]); ta.R = two ? 2 * V : V; ta.C = 1; ta.T = T; ta.srow_mul = nc; ta.srow_add = c;
-                    if (two) { ta.in2 = buf(gn.in_buf[c + 1]); ta.out2 = buf(gn.out_buf[c + 1]); ta.seg_rows = V; }
-                    if (!gn.src_port.empty()) {  // fed by graph_in: rows of the caller's buffer, one voice apart
-                        const float* base = d_in + ck.t0;
-                        ta.in = base + (size_t)gn.src_port[c] * ck.Tfull; if (two) ta.in2 = base + (size_t)gn.src_port[c + 1] * ck.Tfull;
-                        ta.in_pitch = n_in * ck.Tfull; ta.zero_first = ck.zero_first;
-                    }
-                    if (gn.kind == FW_NODE_SVF) { ta.svf = 1; ta.ns = st.params->num_stages; ta.coeffs = st.d_coeffs; ta.state = st.d_state; }
-                    else if (gn.kind == FW_NODE_BIQUAD) { ta.ns = st.params->num_stages; ta.coeffs = st.d_coeffs; ta.state = st.d_state; }
-                    else if (D) { ta.D = D; ta.ring = st.d_ring; ta.pos = st.ring_pos; }
-                    ProfScope ps(p, 3);
-                    if (!FW_CUDA(launch_temporal(ta, p->stream))) return FW_PROC_DEVICE_ERROR;
-                    p->launches++;
-                }
-                if (D) st.ring_pos = (uint32_t)(((uint64_t)st.ring_pos + T) % D);
+            case FW_NODE_SVF: case FW_NODE_BIQUAD: case FW_NODE_DELAY: {
+                NodeDeviceState* st = gn.st.get();
+                rc = run_temporal(p, gn.kind == FW_NODE_DELAY ? nullptr : st, gn.kind == FW_NODE_DELAY ? st : nullptr, node_rows(gn, gn.in_buf.size()), (uint32_t)gn.in_buf.size(), T, zf);
                 break;
             }
-            case FW_NODE_CONV_REVERB: {
-                NodeDeviceState& rs = *gn.st;
-                if (T > NodeDeviceState::kReverbMaxFrames) { g_dev_err = "conv reverb: more than 65536 frames in one chunk"; return FW_PROC_BAD_ARGS; }
-                const uint32_t nc = (uint32_t)gn.in_buf.size(), H = reverb_hist(rs.params->ir_len);
-                if (rs.xh_cursor + T > rs.xh_pitch || (rs.xh_cursor & 7u)) {
-                    if (!FW_CUDA(cudaMemcpy2DAsync(rs.d_xh[rs.xh_cur ^ 1u], (size_t)rs.xh_pitch * 2, static_cast<const uint16_t*>(rs.d_xh[rs.xh_cur]) + (rs.xh_cursor - H),
-                                                   (size_t)rs.xh_pitch * 2, (size_t)H * 2, (size_t)V * nc, cudaMemcpyDeviceToDevice, p->stream))) return FW_PROC_DEVICE_ERROR;
-                    rs.xh_cur ^= 1u; rs.xh_cursor = H;
-                }
-                for (uint32_t c = 0; c < nc; ++c) {
-                    ReverbCall rc{};
-                    rc.in = buf(gn.in_buf[c]); rc.out = buf(gn.out_buf[c]); rc.xh = rs.d_xh[rs.xh_cur]; rc.bt = rs.d_bt;
-                    rc.V = V; rc.C = 1; rc.T = T; rc.L = rs.params->ir_len; rc.ir_ch = rs.params->ir_channels; rc.cursor = rs.xh_cursor; rc.pitch = rs.xh_pitch; rc.chan_base = c;
-                    rc.ws = rs.d_rv_ws; rc.flags = rs.d_rv_flags; rc.epoch = ++rs.rv_epoch;
-                    std::string rerr;
-                    ProfScope ps(p, 3);
-                    if (!FW_CUDA(launch_reverb(rc, p->stream, &rerr))) { if (!rerr.empty()) g_dev_err = rerr; return FW_PROC_DEVICE_ERROR; }
-                    p->launches += 2;
-                }
-                rs.xh_cursor += T;
+            case FW_NODE_CONV_REVERB:
+                rc = run_reverb(p, *gn.st, node_rows(gn, gn.in_buf.size()), (uint32_t)gn.in_buf.size(), T, zf);
                 break;
-            }
             case FW_NODE_CUSTOM: {  // AudioNodeProcessor::process for all voices and blocks at once (fw_node_vtable::process_device)
                 NodeDeviceState& st = *gn.st;
                 const uint32_t nb = (T + pl.block_frames - 1) / pl.block_frames;
@@ -1665,6 +1670,7 @@ static int enqueue_generic(fw_processor* p, Plan& pl, const float* d_in, float* 
             }
             default: g_dev_err = "generic lowering: unknown node kind"; return FW_PROC_DEVICE_ERROR;
         }
+        if (rc != FW_PROC_OK) return rc;
     }
     return FW_PROC_OK;
 }
@@ -1746,8 +1752,7 @@ static int enqueue_chunk(fw_processor* p, Plan& pl, const float* d_in, float* d_
     }
     ca.flags = pl.d_flags; ca.num_voices = V; ca.frames = T; ca.block_frames = pl.block_frames;
     ca.a = p->sm_a; ca.b = p->sm_b; ca.eps = p->sm_eps; ca.err_value = ((p->capturing ? kGraphEpoch : p->call_epoch) << 4) | 1u;
-    { ProfScope ps(p, 0); if (!FW_CUDA(launch_control(ca, p->stream))) return FW_PROC_DEVICE_ERROR; }
-    p->launches++;
+    if (!FW_LAUNCH(p, 0, 1, launch_control(ca, p->stream))) return FW_PROC_DEVICE_ERROR;
 
     if (pl.generic) return enqueue_generic(p, pl, d_in, d_out, ck);
     // ---- data plane: run the stages in order; intermediates ping-pong through [V][ch][Tc] scratch ----
@@ -1758,70 +1763,28 @@ static int enqueue_chunk(fw_processor* p, Plan& pl, const float* d_in, float* d_
         const bool last = si + 1 == n_stages;
         float* dst = last ? d_out + ck.t0 : pl.d_tmp[si & 1];
         const uint32_t dst_pitch = last ? ck.Tfull : T;
-        if (sg.kind == 3) {  // SamplerNode heading the chain: writes [V][c_out][pitch]
-            NodeDeviceState& st = *sg.sampler;
-            SamplerArgs sa{};
-            for (uint32_t c = 0; c < sg.c_out; ++c) sa.out[c] = dst + (size_t)c * dst_pitch;
-            sa.out_vstride = (uint64_t)sg.c_out * dst_pitch; sa.n_out = sg.c_out; sa.num_voices = V; sa.frames = T; sa.block_frames = pl.block_frames;
-            sa.srec = pl.d_srec[0]; sa.res = st.d_res; sa.loop_start = st.d_loop_start; sa.res_tab = st.cur_tab; sa.sm = sg.sampler_sm; sa.rec = pl.rec;
-            { ProfScope ps(p, 1); if (!FW_CUDA(launch_sampler(sa, p->stream))) return FW_PROC_DEVICE_ERROR; }
-            p->launches++;
-            src = dst; src_pitch = dst_pitch;
-            continue;
-        }
-        if (sg.kind == 2) {
-            NodeDeviceState& rs = *sg.reverb;
-            if (T > NodeDeviceState::kReverbMaxFrames) { g_dev_err = "conv reverb: more than 65536 frames in one chunk"; return FW_PROC_BAD_ARGS; }
-            ReverbCall rc{};
-            const uint32_t H = reverb_hist(rs.params->ir_len);
-            if (rs.xh_cursor + T > rs.xh_pitch || (rs.xh_cursor & 7u)) {  // buffer full (or cursor off the 16-byte TMA grid after an odd-length call):
-                // carry the H most recent samples to the front of the other buffer
-                if (!FW_CUDA(cudaMemcpy2DAsync(rs.d_xh[rs.xh_cur ^ 1u], (size_t)rs.xh_pitch * 2, static_cast<const uint16_t*>(rs.d_xh[rs.xh_cur]) + (rs.xh_cursor - H),
-                                               (size_t)rs.xh_pitch * 2, (size_t)H * 2, (size_t)V * sg.c_in, cudaMemcpyDeviceToDevice, p->stream))) return FW_PROC_DEVICE_ERROR;
-                rs.xh_cur ^= 1u; rs.xh_cursor = H;
+        const RowBlock rows{src, dst, sg.c_out, src_pitch, dst_pitch};  // all c_out channels of a non-pointwise stage (c_in: the same or none)
+        const uint32_t zf = si == 0 ? ck.zero_first : 0u;
+        int rc = FW_PROC_OK;
+        switch (sg.kind) {
+            case Plan::STAGE_SAMPLER: rc = run_sampler(p, pl, *sg.node, pl.d_srec[0], sg.sampler_sm, &rows, 1, T); break;
+            case Plan::STAGE_REVERB: rc = run_reverb(p, *sg.node, &rows, 1, T, zf); break;
+            case Plan::STAGE_TEMPORAL: rc = run_temporal(p, sg.node.get(), sg.delay.get(), &rows, 1, T, zf); break;
+            case Plan::STAGE_POINTWISE: {
+                ChainArgs xa{};
+                for (uint32_t c = 0; c < 2; ++c) {  // staged chains read / write [V][ch][pitch]
+                    xa.in_ch[c] = src + (size_t)(c < sg.prog.c_in ? c : 0) * src_pitch;
+                    xa.out_ch[c] = dst + (size_t)(c < sg.prog.c_out ? c : 0) * dst_pitch;
+                }
+                xa.in_vstride = (uint64_t)sg.prog.c_in * src_pitch; xa.out_vstride = (uint64_t)sg.prog.c_out * dst_pitch;
+                xa.num_voices = V; xa.frames = T; xa.block_frames = pl.block_frames; xa.zero_first_block = (si == 0 && ck.zero_first) ? 1u : 0u;
+                xa.rec = pl.rec; xa.prog = sg.prog; xa.in_from_prev_kernel = si > 0 ? 1u : 0u;
+                if (last && pl.bus) rc = run_bus_stage(p, pl, xa, n_out, ck, d_out + ck.t0);
+                else if (!FW_LAUNCH(p, 1, 1, launch_chain(xa, false, p->stream))) rc = FW_PROC_DEVICE_ERROR;
+                break;
             }
-            rc.in = src; rc.out = dst; rc.in_pitch = src_pitch; rc.out_pitch = dst_pitch; rc.xh = rs.d_xh[rs.xh_cur]; rc.bt = rs.d_bt;
-            rc.V = V; rc.C = sg.c_in; rc.T = T; rc.L = rs.params->ir_len; rc.ir_ch = rs.params->ir_channels; rc.cursor = rs.xh_cursor; rc.pitch = rs.xh_pitch;
-            rc.zero_first = si == 0 ? ck.zero_first : 0u; rc.chan_base = 0;
-            rc.ws = rs.d_rv_ws; rc.flags = rs.d_rv_flags; rc.epoch = ++rs.rv_epoch;
-            std::string rerr;
-            { ProfScope ps(p, 3); if (!FW_CUDA(launch_reverb(rc, p->stream, &rerr))) { if (!rerr.empty()) g_dev_err = rerr; return FW_PROC_DEVICE_ERROR; } }
-            p->launches += 2;
-            rs.xh_cursor += T;
-            src = dst; src_pitch = dst_pitch;
-            continue;
         }
-        if (sg.kind == 1) {
-            TemporalArgs ta{};
-            ta.in = src; ta.out = dst; ta.in_pitch = src_pitch; ta.out_pitch = dst_pitch; ta.R = V * sg.c_in; ta.C = sg.c_in; ta.T = T; ta.zero_first = si == 0 ? ck.zero_first : 0u;
-            ta.srow_mul = 1; ta.srow_add = 0;
-            if (sg.biquad) { ta.ns = sg.biquad->params->num_stages; ta.coeffs = sg.biquad->d_coeffs; ta.state = sg.biquad->d_state; }
-            if (sg.svf) { ta.svf = 1; ta.ns = sg.svf->params->num_stages; ta.coeffs = sg.svf->d_coeffs; ta.state = sg.svf->d_state; }
-            if (sg.delay && sg.delay->params->delay) {
-                ta.D = sg.delay->params->delay; ta.ring = sg.delay->d_ring; ta.pos = sg.delay->ring_pos;
-                sg.delay->ring_pos = (uint32_t)(((uint64_t)sg.delay->ring_pos + T) % ta.D);
-            }
-            { ProfScope ps(p, 3); if (!FW_CUDA(launch_temporal(ta, p->stream))) return FW_PROC_DEVICE_ERROR; }
-            p->launches++;
-            src = dst; src_pitch = dst_pitch;
-            continue;
-        }
-        ChainArgs xa{};
-        for (uint32_t c = 0; c < 2; ++c) {  // staged chains read / write [V][ch][pitch]
-            xa.in_ch[c] = src + (size_t)(c < sg.prog.c_in ? c : 0) * src_pitch;
-            xa.out_ch[c] = dst + (size_t)(c < sg.prog.c_out ? c : 0) * dst_pitch;
-        }
-        xa.in_vstride = (uint64_t)sg.prog.c_in * src_pitch; xa.out_vstride = (uint64_t)sg.prog.c_out * dst_pitch;
-        xa.num_voices = V; xa.frames = T; xa.block_frames = pl.block_frames; xa.zero_first_block = (si == 0 && ck.zero_first) ? 1u : 0u;
-        xa.rec = pl.rec; xa.prog = sg.prog; xa.in_from_prev_kernel = si > 0 ? 1u : 0u;
-        if (!(last && pl.bus)) {
-            xa.out = nullptr;
-            { ProfScope ps(p, 1); if (!FW_CUDA(launch_chain(xa, false, p->stream))) return FW_PROC_DEVICE_ERROR; }
-            p->launches++;
-        } else {
-            const int brc = run_bus_stage(p, pl, xa, n_out, ck, d_out + ck.t0);
-            if (brc != FW_PROC_OK) return brc;
-        }
+        if (rc != FW_PROC_OK) return rc;
         src = dst; src_pitch = dst_pitch;
     }
     return FW_PROC_OK;
@@ -1918,7 +1881,7 @@ static int proc_call(fw_processor* p, const float* d_in, float* d_out, uint32_t 
         if (!p->running) { silence_from(b * F); rc = FW_PROC_DROP_PROCESSOR; break; }        // :150-155
         Plan& pl = *p->plan;
         if (n_in != pl.c_in || n_out != pl.c_out) { g_dev_err = "channel counts do not match the compiled graph"; return FW_PROC_BAD_ARGS; }
-        if (b == 0) for (auto& st : pl.states) if (!st->snapshot_params(p->stream)) return FW_PROC_DEVICE_ERROR;
+        if (b == 0) for (auto& st : pl.states) st->snapshot_params();
         while (next_cmd < p->pend_n && p->pend[next_cmd].block < b) ++next_cmd;
         const bool have_cmds = next_cmd < p->pend_n && p->pend[next_cmd].block == b;
         if (have_cmds || !pl.samplers.empty()) { if (!apply_commands(p, pl, b)) return FW_PROC_DEVICE_ERROR; }

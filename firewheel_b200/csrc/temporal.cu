@@ -60,13 +60,12 @@ __device__ __forceinline__ float* row_out(const TemporalArgs& a, const RowMap& m
 //     cooperative copies carry no per-lane predicates or branches.
 //   * SVF = true: the per-stage update is the trapezoidal SVF's (include/fw_b200.h) instead of the TDF-II biquad's; the lane /
 //     tile / pipeline machinery is identical. Coefficient rows are then 6 floats {a1, a2, a3, m0, m1, m2}, state {ic1, ic2}.
-template <int NS, int L, bool DELAY, int RPL, bool FULL, bool SVF = false, int CHF = 32>
+template <int NS, int L, bool DELAY, bool FULL, bool SVF = false, int CHF = 32>
 __global__ void __launch_bounds__(32) biquad_delay_lanes(TemporalArgs a) {
     static_assert(CHF == 32 || CHF == 64, "frames per chunk");
     constexpr uint32_t G = CHF / 4;  // 16-byte granules per tile row
     constexpr uint32_t YM = 1u;                       // y tile slots - 1
-    // RPL rows per lane: each lane runs stage s of RPL independent rows.
-    constexpr int RSET = 32 / L, ROWS = RPL * RSET, PER = RPL * (CHF / 4) / L, LAG = NS > 0 ? 2 * (NS - 1) : 0;
+    constexpr int ROWS = 32 / L, PER = (CHF / 4) / L, LAG = NS > 0 ? 2 * (NS - 1) : 0;
     static_assert(NS <= L && (L == 1 || L == 2 || L == 4 || L == 8), "lanes per row");
     // No early launch_dependents here: this kernel is issue-bound, and dependents parked at griddepcontrol.wait
     // cost it issue slots. The implicit trigger at exit is enough.
@@ -78,24 +77,21 @@ __global__ void __launch_bounds__(32) biquad_delay_lanes(TemporalArgs a) {
     __shared__ float4 rt[DELAY ? 3 : 1][ROWS][G];
     __shared__ float4 yt[2][ROWS][G];
 
-    uint32_t row_l[RPL], rsw[RPL]; bool lane_ok[RPL], last_ok[RPL];
-    float b0[RPL], b1[RPL], b2[RPL], a1[RPL], a2[RPL], c5[RPL], s1[RPL], s2[RPL], q0[RPL], q1[RPL], yb[RPL][4];
-#pragma unroll
-    for (int j = 0; j < RPL; ++j) {
-        row_l[j] = j * RSET + lane / L; rsw[j] = row_l[j] & 7u;
-        const uint32_t r = row0 + row_l[j];
-        lane_ok[j] = (FULL || r < R) && (NS == 0 ? s == 0 : s < (uint32_t)NS);
-        last_ok[j] = is_last && lane_ok[j];
-        b0[j] = b1[j] = b2[j] = a1[j] = a2[j] = c5[j] = s1[j] = s2[j] = q0[j] = q1[j] = 0.0f;
-        yb[j][0] = yb[j][1] = yb[j][2] = yb[j][3] = 0.0f;
-        if (NS > 0 && lane_ok[j]) {
-            const RowMap rm = row_map(a, r);
-            const float* k = a.coeffs + ((size_t)(rm.rr / a.C) * NS + s) * (SVF ? 6 : 5);
-            b0[j] = k[0]; b1[j] = k[1]; b2[j] = k[2]; a1[j] = k[3]; a2[j] = k[4];
-            if (SVF) c5[j] = k[5];
-            const size_t sr = rm.srow;
-            s1[j] = a.state[(sr * kStateStages + s) * 2]; s2[j] = a.state[(sr * kStateStages + s) * 2 + 1];
-        }
+    uint32_t row_l, rsw; bool lane_ok, last_ok;
+    float b0, b1, b2, a1, a2, c5, s1, s2, q0, q1, yb[4];
+    row_l = lane / L; rsw = row_l & 7u;  // this lane's row inside the CTA
+    const uint32_t r = row0 + row_l;
+    lane_ok = (FULL || r < R) && (NS == 0 ? s == 0 : s < (uint32_t)NS);
+    last_ok = is_last && lane_ok;
+    b0 = b1 = b2 = a1 = a2 = c5 = s1 = s2 = q0 = q1 = 0.0f;
+    yb[0] = yb[1] = yb[2] = yb[3] = 0.0f;
+    if (NS > 0 && lane_ok) {
+        const RowMap rm = row_map(a, r);
+        const float* k = a.coeffs + ((size_t)(rm.rr / a.C) * NS + s) * (SVF ? 6 : 5);
+        b0 = k[0]; b1 = k[1]; b2 = k[2]; a1 = k[3]; a2 = k[4];
+        if (SVF) c5 = k[5];
+        const size_t sr = rm.srow;
+        s1 = a.state[(sr * kStateStages + s) * 2]; s2 = a.state[(sr * kStateStages + s) * 2 + 1];
     }
     // cooperative copies: lane handles PER (row, granule) pairs of every tile
     const float* in_p[PER]; float* out_p[PER]; float* ring_p[PER]; uint32_t sw[PER]; bool ok[PER], hi[PER];
@@ -141,87 +137,64 @@ __global__ void __launch_bounds__(32) biquad_delay_lanes(TemporalArgs a) {
         if (DELAY) advance(ring_flush_off);
     };
 
-    // One skewed iteration of all RPL rows; gi = global iteration index, u4 = gi & 3 (compile-time when unrolled).
+    // One skewed iteration of this lane's row; gi = global iteration index, u4 = gi & 3 (compile-time when unrolled).
     // q0/q1: inter-stage pipeline — the value shuffled in iteration n is the input of iteration n+2.
     // CHECK = true (first chunk, zeroed chunks, drain): stage s is live only while its sample n = gi - 2s is in [0, T).
     // CHECK = false (every other chunk): all stages are live; lanes that own no stage run on garbage that is never stored.
-    // per-lane swizzled granule offsets of this lane's row(s) inside a tile row: granule c lives at c ^ (row & 7)
-    uint32_t goff[RPL][G];
+    // per-lane swizzled granule offsets of this lane's row inside a tile row: granule c lives at c ^ (row & 7)
+    uint32_t goff[G];
 #pragma unroll
-    for (int j = 0; j < RPL; ++j)
-#pragma unroll
-        for (int c = 0; c < (int)G; ++c) goff[j][c] = (uint32_t)c ^ rsw[j];
-    const float4* xbase[RPL] = {}; float4* ybase[RPL][2] = {};  // refreshed per chunk: x tile row, y tile rows of this / the previous chunk
-    auto body = [&](auto check, uint32_t gi, const float (&x)[RPL], int u4, int n4) {
+    for (int c = 0; c < (int)G; ++c) goff[c] = (uint32_t)c ^ rsw;
+    const float4* xbase = nullptr; float4* ybase[2] = {};  // refreshed per chunk: x tile row, y tile rows of this / the previous chunk
+    auto body = [&](auto check, uint32_t gi, float x, int u4, int n4) {
         constexpr bool CHECK = decltype(check)::value;
         const bool in_range = CHECK ? (gi - 2u * s) < T : true;  // unsigned compare: also false during warm-up (gi < 2s)
         const int slot = (u4 - LAG) & 3;  // the last stage emits sample m = gi - LAG; (gi - LAG) & 3 == (u4 - LAG) & 3
-#pragma unroll
-        for (int j = 0; j < RPL; ++j) {
-            const bool active = CHECK ? (lane_ok[j] && in_range) : true;
-            float y;
-            if (NS == 0) {
-                y = x[j];
+        const bool active = CHECK ? (lane_ok && in_range) : true;
+        float y;
+        if (NS == 0) {
+            y = x;
+        } else {
+            const float xi = is_first ? x : q0;
+            float n1, n2;
+            if (SVF) {  // (b0, b1, b2, a1, a2, c5) hold (a1, a2, a3, m0, m1, m2); (s1, s2) hold (ic1, ic2)
+                const float v3 = __fsub_rn(xi, s2);
+                const float v1 = __fadd_rn(__fmul_rn(b0, s1), __fmul_rn(b1, v3));
+                const float v2 = __fadd_rn(s2, __fadd_rn(__fmul_rn(b1, s1), __fmul_rn(b2, v3)));
+                n1 = __fsub_rn(__fmul_rn(2.0f, v1), s1);
+                n2 = __fsub_rn(__fmul_rn(2.0f, v2), s2);
+                y = __fadd_rn(__fmul_rn(a1, xi), __fadd_rn(__fmul_rn(a2, v1), __fmul_rn(c5, v2)));
             } else {
-                const float xi = is_first ? x[j] : q0[j];
-                float n1, n2;
-                if (SVF) {  // (b0, b1, b2, a1, a2, c5) hold (a1, a2, a3, m0, m1, m2); (s1, s2) hold (ic1, ic2)
-                    const float v3 = __fsub_rn(xi, s2[j]);
-                    const float v1 = __fadd_rn(__fmul_rn(b0[j], s1[j]), __fmul_rn(b1[j], v3));
-                    const float v2 = __fadd_rn(s2[j], __fadd_rn(__fmul_rn(b1[j], s1[j]), __fmul_rn(b2[j], v3)));
-                    n1 = __fsub_rn(__fmul_rn(2.0f, v1), s1[j]);
-                    n2 = __fsub_rn(__fmul_rn(2.0f, v2), s2[j]);
-                    y = __fadd_rn(__fmul_rn(a1[j], xi), __fadd_rn(__fmul_rn(a2[j], v1), __fmul_rn(c5[j], v2)));
-                } else {
-                    y = __fadd_rn(__fmul_rn(b0[j], xi), s1[j]);
-                    n1 = __fadd_rn(__fsub_rn(__fmul_rn(b1[j], xi), __fmul_rn(a1[j], y)), s2[j]);
-                    n2 = __fsub_rn(__fmul_rn(b2[j], xi), __fmul_rn(a2[j], y));
-                }
-                if (!CHECK || active) { s1[j] = n1; s2[j] = n2; }
-                q0[j] = q1[j];
-                q1[j] = __shfl_up_sync(0xffffffffu, y, 1);
+                y = __fadd_rn(__fmul_rn(b0, xi), s1);
+                n1 = __fadd_rn(__fsub_rn(__fmul_rn(b1, xi), __fmul_rn(a1, y)), s2);
+                n2 = __fsub_rn(__fmul_rn(b2, xi), __fmul_rn(a2, y));
             }
-            yb[j][slot] = y;
-            if (slot == 3 && (CHECK ? (is_last && active) : last_ok[j])) {
-                // m = gi - LAG lies in this chunk iff n4 * 4 + u4 >= LAG (all compile-time); granule (m >> 2) & 7
-                const int ml = n4 * 4 + u4 - LAG;
-                ybase[j][ml >= 0 ? 0 : 1][goff[j][(ml >> 2) & (int)(G - 1)]] = make_float4(yb[j][0], yb[j][1], yb[j][2], yb[j][3]);
-            }
+            if (!CHECK || active) { s1 = n1; s2 = n2; }
+            q0 = q1;
+            q1 = __shfl_up_sync(0xffffffffu, y, 1);
+        }
+        yb[slot] = y;
+        if (slot == 3 && (CHECK ? (is_last && active) : last_ok)) {
+            // m = gi - LAG lies in this chunk iff n4 * 4 + u4 >= LAG (all compile-time); granule (m >> 2) & 7
+            const int ml = n4 * 4 + u4 - LAG;
+            ybase[ml >= 0 ? 0 : 1][goff[(ml >> 2) & (int)(G - 1)]] = make_float4(yb[0], yb[1], yb[2], yb[3]);
         }
     };
     auto chunk = [&](auto check, uint32_t ch, bool zero_in) {
-#pragma unroll
-        for (int j = 0; j < RPL; ++j) {
-            xbase[j] = &xt[ch & 3u][row_l[j]][0];
-            ybase[j][0] = &yt[ch & YM][row_l[j]][0];
-            ybase[j][1] = &yt[(ch + YM) & YM][row_l[j]][0];
-        }
-        float4 xnext[RPL];  // software-pipelined: the LDS.128 for step n4+1 is issued before step n4 is consumed
-#pragma unroll
-        for (int j = 0; j < RPL; ++j) xnext[j] = xbase[j][goff[j][0]];
+        xbase = &xt[ch & 3u][row_l][0];
+        ybase[0] = &yt[ch & YM][row_l][0];
+        ybase[1] = &yt[(ch + YM) & YM][row_l][0];
+        float4 xnext = xbase[goff[0]];  // software-pipelined: the LDS.128 for step n4+1 is issued before step n4 is consumed
 #pragma unroll
         for (uint32_t n4 = 0; n4 < G; ++n4) {
-            float4 xq[RPL];  // every lane of a row reads the same granule (broadcast); only stage 0 uses it
-#pragma unroll
-            for (int j = 0; j < RPL; ++j) {
-                xq[j] = xnext[j];
-                if (n4 + 1u < G) xnext[j] = xbase[j][goff[j][(n4 + 1u) & (G - 1u)]];
-                if (decltype(check)::value && zero_in) xq[j] = make_float4(0.0f, 0.0f, 0.0f, 0.0f);
-            }
+            float4 xq = xnext;  // every lane of a row reads the same granule (broadcast); only stage 0 uses it
+            if (n4 + 1u < G) xnext = xbase[goff[(n4 + 1u) & (G - 1u)]];
+            if (decltype(check)::value && zero_in) xq = make_float4(0.0f, 0.0f, 0.0f, 0.0f);
             const uint32_t gi = ch * (uint32_t)CHF + n4 * 4u;
-            float x[RPL];
-#pragma unroll
-            for (int j = 0; j < RPL; ++j) x[j] = xq[j].x;
-            body(check, gi, x, 0, (int)n4);
-#pragma unroll
-            for (int j = 0; j < RPL; ++j) x[j] = xq[j].y;
-            body(check, gi + 1u, x, 1, (int)n4);
-#pragma unroll
-            for (int j = 0; j < RPL; ++j) x[j] = xq[j].z;
-            body(check, gi + 2u, x, 2, (int)n4);
-#pragma unroll
-            for (int j = 0; j < RPL; ++j) x[j] = xq[j].w;
-            body(check, gi + 3u, x, 3, (int)n4);
+            body(check, gi, xq.x, 0, (int)n4);
+            body(check, gi + 1u, xq.y, 1, (int)n4);
+            body(check, gi + 2u, xq.z, 2, (int)n4);
+            body(check, gi + 3u, xq.w, 3, (int)n4);
         }
     };
 
@@ -244,23 +217,18 @@ __global__ void __launch_bounds__(32) biquad_delay_lanes(TemporalArgs a) {
         else chunk(std::false_type{}, ch, false);
     }
     if (nch > 0) {
-        const float zx[RPL] = {};
+        ybase[0] = &yt[nch & YM][row_l][0]; ybase[1] = &yt[(nch + YM) & YM][row_l][0];
 #pragma unroll
-        for (int j = 0; j < RPL; ++j) { ybase[j][0] = &yt[nch & YM][row_l[j]][0]; ybase[j][1] = &yt[(nch + YM) & YM][row_l[j]][0]; }
-#pragma unroll
-        for (int it = 0; it < ((LAG + 3) & ~3); ++it) body(std::true_type{}, T + it, zx, it & 3, it >> 2);  // drain (T % 4 == 0)
+        for (int it = 0; it < ((LAG + 3) & ~3); ++it) body(std::true_type{}, T + it, 0.0f, it & 3, it >> 2);  // drain (T % 4 == 0)
         __syncwarp();
         if (nch >= 2u) flush_y(nch - 2u);
         flush_y(nch - 1u);
     }
     cp_async_wait<0>();
-#pragma unroll
-    for (int j = 0; j < RPL; ++j) {
-        if (NS > 0 && lane_ok[j]) {
-            const size_t sr = row_map(a, row0 + row_l[j]).srow;
-            a.state[(sr * kStateStages + s) * 2] = s1[j];
-            a.state[(sr * kStateStages + s) * 2 + 1] = s2[j];
-        }
+    if (NS > 0 && lane_ok) {
+        const size_t sr = row_map(a, row0 + row_l).srow;
+        a.state[(sr * kStateStages + s) * 2] = s1;
+        a.state[(sr * kStateStages + s) * 2 + 1] = s2;
     }
 }
 
@@ -336,18 +304,18 @@ static cudaError_t launch_pdl_t(void (*kernel)(KArgs...), dim3 grid, dim3 block,
     return cudaLaunchKernelEx(&cfg, kernel, std::forward<Args>(args)...);
 }
 
-// Full CTAs of one row per lane + predicated CTAs for the ragged tail.
+// Full CTAs + predicated CTAs for the ragged tail.
 template <int NS, int L, bool DELAY, bool SVF, int CHF>
 static cudaError_t launch_lanes_c(const TemporalArgs& a, cudaStream_t st) {
     constexpr uint32_t rows1 = 32 / L;
     const uint32_t n_full = a.R / rows1, done = n_full * rows1;
     if (n_full) {
-        cudaError_t e = launch_pdl_t(biquad_delay_lanes<NS, L, DELAY, 1, true, SVF, CHF>, dim3(n_full), dim3(32), st, a);
+        cudaError_t e = launch_pdl_t(biquad_delay_lanes<NS, L, DELAY, true, SVF, CHF>, dim3(n_full), dim3(32), st, a);
         if (e != cudaSuccess) return e;
     }
     if (done < a.R) {  // ragged tail
         TemporalArgs t = a; t.row_base = done;
-        return launch_pdl_t(biquad_delay_lanes<NS, L, DELAY, 1, false, SVF, 32>, dim3((a.R - done + rows1 - 1) / rows1), dim3(32), st, t);
+        return launch_pdl_t(biquad_delay_lanes<NS, L, DELAY, false, SVF, 32>, dim3((a.R - done + rows1 - 1) / rows1), dim3(32), st, t);
     }
     return cudaSuccess;
 }
