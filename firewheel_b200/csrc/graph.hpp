@@ -91,11 +91,10 @@ struct NodeParams;
 enum CmdKind : uint32_t {
     CMD_SAMPLER = 0,   // a = SmpMsgKind, x / y / b = payload (NodeToProcessorMsg sampler.rs:21-28)
     CMD_TARGET = 1,    // a = smoothed-parameter index of the node (0: raw_gain / gain_l, 1: gain_r), f[0] = value
-    CMD_BIQUAD = 2,    // a = stage, f[0..4] = {b0, b1, b2, a1, a2}
-    CMD_SVF = 3,       // a = stage, f[0..5] = {a1, a2, a3, m0, m1, m2}
-    CMD_RS_SET = 4,    // b = resource, x = step (Q32.32), a = flags (bit0 playing, bit1 loop)
-    CMD_RS_SEEK = 5,   // x = position in frames
-    CMD_UPLOAD = 6     // a whole parameter array at once (set_percent_volumes, set_all_coeffs ...): a = array (0 / 1: smoothed target 0 / 1,
+    CMD_COEFFS = 2,    // a = stage, f[0 .. coeff_width(kind)) = that stage's biquad or SVF coefficients (see NodeParams::coeffs)
+    CMD_RS_SET = 3,    // b = resource, x = step (Q32.32), a = flags (bit0 playing, bit1 loop)
+    CMD_RS_SEEK = 4,   // x = position in frames
+    CMD_UPLOAD = 5     // a whole parameter array at once (set_percent_volumes, set_all_coeffs ...): a = array (0 / 1: smoothed target 0 / 1,
                        // 2: coefficient table), x = float* snapshot taken by the main thread (handed back through Channels::to_free), y = floats
 };
 struct Cmd { uint32_t kind, block, voice /* or FW_ALL_VOICES */, a, b, pad; uint64_t x, y; float f[6]; const NodeParams* node; };
@@ -113,16 +112,15 @@ struct NodeParams {
     std::vector<float> pan, gain_l, gain_r;
     // hard clip (hard_clip.rs:8-12)
     float threshold_gain = 0.0f;
-    // biquad
+    // biquad and SVF (spec ours): [voice][stage][coeff_width(kind)], a biquad stage {b0, b1, b2, a1, a2}, an SVF stage
+    // {a1, a2, a3, m0, m1, m2}
     uint32_t num_stages = 0;
-    std::vector<float> coeffs;  // [voice][stage][5]
+    std::vector<float> coeffs;
     // delay
     uint32_t delay = 0;
     // conv reverb
     uint32_t ir_len = 0, ir_channels = 0;
     std::vector<float> ir;  // [ch][len] f32 (rounded to bf16 on the device side)
-    // svf (spec ours): [voice][stage][6] = {a1, a2, a3, m0, m1, m2}; num_stages above
-    std::vector<float> svf_coeffs;
     // polyphase resampler (spec ours): table [phases][taps]; the per-voice transport travels as commands
     uint32_t rs_phases = 0, rs_taps = 0; std::vector<float> rs_table;
     // sampler (sampler.rs:46-181): node-side state per voice (main thread only). `percent` / `raw_gain` above double as the
@@ -132,6 +130,8 @@ struct NodeParams {
     std::vector<uint16_t> smp_pending;     // messages queued per voice since the stream side last drained (ring capacity 128, sampler.rs:14)
     std::vector<uint32_t> smp_pending_epoch;  // drain epoch `smp_pending[v]` was counted in
 };
+// floats per stage in NodeParams::coeffs: 5 for a biquad, 6 for an SVF, 0 for a node without a coefficient table
+inline uint32_t coeff_width(uint32_t kind) { return kind == FW_NODE_BIQUAD ? 5 : kind == FW_NODE_SVF ? 6 : 0; }
 
 const char* node_debug_name(uint32_t kind);
 // AudioNodeInfo per kind (node.rs:57-79 as filled in by each basic node)

@@ -49,13 +49,36 @@ static bool cuda_ok(cudaError_t e, const char* what) {
 }
 #define FW_CUDA(call) fw::cuda_ok((call), #call)
 
-template <class T> static T* dev_alloc(size_t n, bool zero = true) {
-    void* p = nullptr;
-    if (n == 0) n = 1;
-    if (!FW_CUDA(cudaMalloc(&p, n * sizeof(T)))) return nullptr;
-    if (zero) cudaMemset(p, 0, n * sizeof(T));
-    return static_cast<T*>(p);
-}
+// Owner of the device and pinned host memory of one runtime object (ResTable, NodeDeviceState, Plan, fw_processor): everything it
+// hands out is freed, on its device, when it is destroyed. The objects keep plain pointers, which travel by value in the kernel
+// arguments. ok() turns false for good at the first failed allocation or zero fill, so a run of allocations is checked once.
+class DevMem {
+  public:
+    const int device;
+    explicit DevMem(int dev) : device(dev) {}
+    DevMem(const DevMem&) = delete; DevMem& operator=(const DevMem&) = delete;
+    ~DevMem() { cudaSetDevice(device); for (void* q : dev_) cudaFree(q); for (void* q : host_) cudaFreeHost(q); }
+    bool ok() const { return ok_; }
+    // n elements (at least one), zero-filled unless `zero` is false
+    template <class T> T* dev(size_t n, bool zero = true) {
+        void* p = nullptr;
+        if (n == 0) n = 1;
+        if (!FW_CUDA(cudaMalloc(&p, n * sizeof(T)))) return failed();
+        dev_.push_back(p);
+        if (zero && !FW_CUDA(cudaMemset(p, 0, n * sizeof(T)))) return failed();
+        return static_cast<T*>(p);
+    }
+    template <class T> T* host(size_t n) {
+        void* p = nullptr;
+        if (!FW_CUDA(cudaMallocHost(&p, n * sizeof(T)))) return failed();
+        host_.push_back(p);
+        return static_cast<T*>(p);
+    }
+  private:
+    // the message stays in g_dev_err; the runtime's pending error is cleared so that the next launch check does not report it
+    std::nullptr_t failed() { cudaGetLastError(); ok_ = false; return nullptr; }
+    std::vector<void*> dev_, host_; bool ok_ = true;
+};
 
 // wait-free SPSC ring (rtrb::RingBuffer, context.rs:61-64), capacity 16
 template <class T, size_t N = 16> struct Spsc {
@@ -93,20 +116,20 @@ template <class T> struct DynSpsc {
 
 // Sample resources of one context ("Arc<dyn SampleResource>", sample_resource.rs): uploaded once, referenced by handle.
 struct ResTable {
-    int device = 0; std::mutex mu;
-    std::vector<ResDesc> host; std::vector<void*> allocs;  // descriptors and the device copies of the sample data
-    ResDesc* d_tab = nullptr; std::vector<void*> retired;   // device table (re-built on every add; old ones stay valid for in-flight calls)
-    ~ResTable() { cudaSetDevice(device); for (void* q : allocs) cudaFree(q); for (void* q : retired) cudaFree(q); cudaFree(d_tab); }
+    std::mutex mu;
+    DevMem mem;  // the device copies of the sample data and every device table (old ones stay valid for in-flight calls)
+    std::vector<ResDesc> host; ResDesc* d_tab = nullptr;  // descriptors and their device table (re-built on every add)
+    explicit ResTable(int device) : mem(device) {}
     uint32_t add(uint32_t fmt, uint32_t channels, uint64_t frames, const void* data) {
         const size_t bytes = (size_t)channels * frames * (fmt <= FW_SAMPLE_F32_INTERLEAVED ? 4 : 2);
-        cudaSetDevice(device);
-        void* d = nullptr;
-        if (!FW_CUDA(cudaMalloc(&d, bytes)) || !FW_CUDA(cudaMemcpy(d, data, bytes, cudaMemcpyHostToDevice))) { cudaFree(d); return 0; }
+        cudaSetDevice(mem.device);
+        uint8_t* d;
+        { std::lock_guard<std::mutex> lk(mu); d = mem.dev<uint8_t>(bytes, false); }  // the upload below runs outside the lock
+        if (!d || !FW_CUDA(cudaMemcpy(d, data, bytes, cudaMemcpyHostToDevice))) return 0;
         std::lock_guard<std::mutex> lk(mu);
-        allocs.push_back(d); host.push_back(ResDesc{d, frames, channels, fmt});
-        ResDesc* nt = nullptr;
-        if (!FW_CUDA(cudaMalloc(&nt, sizeof(ResDesc) * host.size())) || !FW_CUDA(cudaMemcpy(nt, host.data(), sizeof(ResDesc) * host.size(), cudaMemcpyHostToDevice))) { cudaFree(nt); host.pop_back(); return 0; }
-        if (d_tab) retired.push_back(d_tab);
+        host.push_back(ResDesc{d, frames, channels, fmt});
+        ResDesc* nt = mem.dev<ResDesc>(host.size(), false);
+        if (!nt || !FW_CUDA(cudaMemcpy(nt, host.data(), sizeof(ResDesc) * host.size(), cudaMemcpyHostToDevice))) { host.pop_back(); return 0; }
         d_tab = nt;
         return (uint32_t)host.size();
     }
@@ -115,7 +138,8 @@ struct ResTable {
 };
 
 struct NodeDeviceState {
-    int device = 0; uint32_t kind = 0, V = 0, n_sm = 0;
+    DevMem mem;  // every buffer below
+    uint32_t kind = 0, V = 0, n_sm = 0;
     std::shared_ptr<NodeParams> params;
     float* d_target[2] = {nullptr, nullptr};      // volume: raw_gain; pan: gain_l, gain_r
     float* sm_input[2] = {nullptr, nullptr};
@@ -123,7 +147,7 @@ struct NodeDeviceState {
     uint32_t* sm_status[2] = {nullptr, nullptr};
     // temporal nodes: `channels` rows per voice
     uint32_t channels = 0;
-    float* d_coeffs = nullptr;   // biquad [V][ns][5]
+    float* d_coeffs = nullptr;   // biquad / SVF [V][ns][coeff_width(kind)]
     float* d_state = nullptr;    // biquad [V*channels][8][2]
     float* d_ring = nullptr;     // delay  [V*channels][D]
     uint32_t ring_pos = 0;       // stream-side cursor into the ring
@@ -141,72 +165,61 @@ struct NodeDeviceState {
     const ResDesc* cur_tab = nullptr; uint32_t cur_n_res = 0;
     // custom node (plugin vtable): the processor returned by activate() and the dense per-(block, voice) input masks handed to it
     void* custom_proc = nullptr; bool custom_deactivate = false;  // true: released through deactivate(node, processor) (graph.rs:603-609,644-648)
-    ~NodeDeviceState() {
-        cudaSetDevice(device);
+    explicit NodeDeviceState(int device) : mem(device) {}
+    ~NodeDeviceState() {  // the plugin lets go of its processor before `mem` frees the node's buffers
+        cudaSetDevice(mem.device);
         if (params && params->custom && custom_proc) {  // main thread: plans are released in ctx_drain / ctx_free
             const fw_node_vtable& vt = params->custom->vt;
             if (custom_deactivate && vt.deactivate) vt.deactivate(params->custom->node, custom_proc);
             else if (vt.drop_processor) vt.drop_processor(custom_proc);
         }
-        for (int i = 0; i < 2; ++i) { cudaFree(d_target[i]); cudaFree(sm_input[i]); cudaFree(sm_last[i]); cudaFree(sm_status[i]); }
-        cudaFree(d_coeffs); cudaFree(d_state); cudaFree(d_ring); cudaFree(d_bt); cudaFree(d_xh[0]); cudaFree(d_xh[1]); cudaFree(d_rv_ws); cudaFree(d_rv_flags);
-        cudaFree(d_playing); cudaFree(d_playhead); cudaFree(d_loop_flags); cudaFree(d_loop_start); cudaFree(d_loop_end); cudaFree(d_res);
-        cudaFree(d_msgs); cudaFree(d_msg_off); cudaFreeHost(h_msgs); cudaFreeHost(h_off); cudaFreeHost(h_cnt); if (ev_staged) cudaEventDestroy(ev_staged);
-        cudaFree(d_rs_table); cudaFree(d_rs_res); cudaFree(d_rs_flags); cudaFree(d_rs_step); cudaFree(d_rs_pos);
+        if (ev_staged) cudaEventDestroy(ev_staged);
     }
     const std::vector<float>& host_target(int i) const { return (kind == FW_NODE_VOLUME || kind == FW_NODE_SAMPLER) ? params->raw_gain : (i == 0 ? params->gain_l : params->gain_r); }
     // ParamSmoother::new(val): input = last_output = val, Inactive (smoother.rs:93-112; volume.rs:67-75)
     bool create() {
         n_sm = (kind == FW_NODE_VOLUME || kind == FW_NODE_SAMPLER) ? 1 : kind == FW_NODE_PAN ? 2 : 0;
         for (uint32_t i = 0; i < n_sm; ++i) {
-            d_target[i] = dev_alloc<float>(V); sm_input[i] = dev_alloc<float>(V); sm_last[i] = dev_alloc<float>(V); sm_status[i] = dev_alloc<uint32_t>(V);
-            if (!d_target[i] || !sm_input[i] || !sm_last[i] || !sm_status[i]) return false;
+            d_target[i] = mem.dev<float>(V); sm_input[i] = mem.dev<float>(V); sm_last[i] = mem.dev<float>(V); sm_status[i] = mem.dev<uint32_t>(V);
+            if (!mem.ok()) return false;
             const float* h = host_target(i).data();
             if (!FW_CUDA(cudaMemcpy(d_target[i], h, V * 4, cudaMemcpyHostToDevice))) return false;
             if (!FW_CUDA(cudaMemcpy(sm_input[i], h, V * 4, cudaMemcpyHostToDevice))) return false;
             if (!FW_CUDA(cudaMemcpy(sm_last[i], h, V * 4, cudaMemcpyHostToDevice))) return false;
         }
-        if (kind == FW_NODE_BIQUAD) {
-            d_coeffs = dev_alloc<float>((size_t)V * params->num_stages * 5, false);
-            d_state = dev_alloc<float>((size_t)V * channels * 8 * 2);  // zero state
-            if (!d_coeffs || !d_state) return false;
+        if (const uint32_t w = coeff_width(kind)) {  // biquad / SVF
+            d_coeffs = mem.dev<float>((size_t)V * params->num_stages * w, false);
+            d_state = mem.dev<float>((size_t)V * channels * 8 * 2);  // zero state
+            if (!mem.ok()) return false;
             if (params->num_stages && !FW_CUDA(cudaMemcpy(d_coeffs, params->coeffs.data(), params->coeffs.size() * 4, cudaMemcpyHostToDevice))) return false;
         } else if (kind == FW_NODE_DELAY && params->delay) {
-            d_ring = dev_alloc<float>((size_t)V * channels * params->delay);  // zero-initialised ring
-            if (!d_ring) return false;
+            d_ring = mem.dev<float>((size_t)V * channels * params->delay);  // zero-initialised ring
+            if (!mem.ok()) return false;
         } else if (kind == FW_NODE_CONV_REVERB) {
             const uint32_t L = params->ir_len, ich = params->ir_channels, kpad = reverb_kpad(L);
             xh_pitch = reverb_hist(L) + kReverbMaxFrames; xh_cursor = reverb_hist(L);
-            d_bt = dev_alloc<uint16_t>((size_t)ich * 256 * kpad, false);
-            d_xh[0] = dev_alloc<uint16_t>((size_t)V * channels * xh_pitch);  // zero history
-            d_xh[1] = dev_alloc<uint16_t>((size_t)V * channels * xh_pitch);
-            float* d_ir = dev_alloc<float>((size_t)ich * L, false);
-            d_rv_ws = dev_alloc<float>(reverb_ws_bytes() / sizeof(float), false); d_rv_flags = dev_alloc<uint32_t>(reverb_grid_max());
-            if (!d_bt || !d_xh[0] || !d_xh[1] || !d_ir || !d_rv_ws || !d_rv_flags) { cudaFree(d_ir); return false; }
-            bool ok = FW_CUDA(cudaMemcpy(d_ir, params->ir.data(), (size_t)ich * L * 4, cudaMemcpyHostToDevice)) &&
-                      FW_CUDA(launch_reverb_build(d_ir, d_bt, L, ich, nullptr)) && FW_CUDA(cudaDeviceSynchronize());
-            cudaFree(d_ir);
-            if (!ok) return false;
-        }
-        if (kind == FW_NODE_SVF) {
-            d_coeffs = dev_alloc<float>((size_t)V * params->num_stages * 6, false);
-            d_state = dev_alloc<float>((size_t)V * channels * 8 * 2);  // zero state
-            if (!d_coeffs || !d_state) return false;
-            if (params->num_stages && !FW_CUDA(cudaMemcpy(d_coeffs, params->svf_coeffs.data(), params->svf_coeffs.size() * 4, cudaMemcpyHostToDevice))) return false;
+            d_bt = mem.dev<uint16_t>((size_t)ich * 256 * kpad, false);
+            d_xh[0] = mem.dev<uint16_t>((size_t)V * channels * xh_pitch);  // zero history
+            d_xh[1] = mem.dev<uint16_t>((size_t)V * channels * xh_pitch);
+            d_rv_ws = mem.dev<float>(reverb_ws_bytes() / sizeof(float), false); d_rv_flags = mem.dev<uint32_t>(reverb_grid_max());
+            DevMem tmp(mem.device);  // the f32 IR, only needed to build d_bt
+            float* d_ir = tmp.dev<float>((size_t)ich * L, false);
+            if (!mem.ok() || !tmp.ok()) return false;
+            return FW_CUDA(cudaMemcpy(d_ir, params->ir.data(), (size_t)ich * L * 4, cudaMemcpyHostToDevice)) &&
+                   FW_CUDA(launch_reverb_build(d_ir, d_bt, L, ich, nullptr)) && FW_CUDA(cudaDeviceSynchronize());
         }
         if (kind == FW_NODE_RESAMPLER) {
-            d_rs_table = dev_alloc<float>(params->rs_table.size(), false);
-            d_rs_res = dev_alloc<uint32_t>(V); d_rs_flags = dev_alloc<uint32_t>(V); d_rs_step = dev_alloc<uint64_t>(V);
-            d_rs_pos = dev_alloc<uint64_t>(V);
-            if (!d_rs_table || !d_rs_res || !d_rs_flags || !d_rs_step || !d_rs_pos) return false;
+            d_rs_table = mem.dev<float>(params->rs_table.size(), false);
+            d_rs_res = mem.dev<uint32_t>(V); d_rs_flags = mem.dev<uint32_t>(V); d_rs_step = mem.dev<uint64_t>(V);
+            d_rs_pos = mem.dev<uint64_t>(V);
+            if (!mem.ok()) return false;
             if (!FW_CUDA(cudaMemcpy(d_rs_table, params->rs_table.data(), params->rs_table.size() * 4, cudaMemcpyHostToDevice))) return false;
             std::vector<uint64_t> one((size_t)V, 1ull << 32);  // step 1.0 until set; not playing, no resource (zero-initialised)
             return FW_CUDA(cudaMemcpy(d_rs_step, one.data(), (size_t)V * 8, cudaMemcpyHostToDevice));
         }
         if (kind == FW_NODE_SAMPLER) {  // SamplerProcessor::new (sampler.rs:300-320): not playing, playhead 0, no loop, no sample
-            d_playing = dev_alloc<uint32_t>(V); d_playhead = dev_alloc<uint64_t>(V); d_loop_flags = dev_alloc<uint32_t>(V);
-            d_loop_start = dev_alloc<uint64_t>(V); d_loop_end = dev_alloc<uint64_t>(V); d_res = dev_alloc<uint32_t>(V); d_msg_off = dev_alloc<uint32_t>((size_t)V + 1);
-            if (!d_playing || !d_playhead || !d_loop_flags || !d_loop_start || !d_loop_end || !d_res || !d_msg_off) return false;
+            d_playing = mem.dev<uint32_t>(V); d_playhead = mem.dev<uint64_t>(V); d_loop_flags = mem.dev<uint32_t>(V);
+            d_loop_start = mem.dev<uint64_t>(V); d_loop_end = mem.dev<uint64_t>(V); d_res = mem.dev<uint32_t>(V); d_msg_off = mem.dev<uint32_t>((size_t)V + 1);
             if (!alloc_sampler_staging(std::max<size_t>(4096, 4 * (size_t)V))) return false;
             params->smp_active = true;  // activate() creates the rings (sampler.rs:204-212)
             std::fill(params->smp_pending.begin(), params->smp_pending.end(), (uint16_t)0);
@@ -219,9 +232,9 @@ struct NodeDeviceState {
     SamplerMsgDev* h_msgs = nullptr; uint32_t* h_off = nullptr; uint32_t* h_cnt = nullptr; cudaEvent_t ev_staged = nullptr; bool staged_pending = false;
     bool alloc_sampler_staging(size_t cap) {
         cap_msgs = cap;
-        return FW_CUDA(cudaMallocHost(&h_msgs, cap * sizeof(SamplerMsgDev))) && FW_CUDA(cudaMallocHost(&h_off, ((size_t)V + 1) * sizeof(uint32_t))) &&
-               FW_CUDA(cudaMallocHost(&h_cnt, ((size_t)V + 1) * sizeof(uint32_t))) && FW_CUDA(cudaMalloc(&d_msgs, cap * sizeof(SamplerMsgDev))) &&
-               FW_CUDA(cudaEventCreateWithFlags(&ev_staged, cudaEventDisableTiming));
+        h_msgs = mem.host<SamplerMsgDev>(cap); h_off = mem.host<uint32_t>((size_t)V + 1); h_cnt = mem.host<uint32_t>((size_t)V + 1);
+        d_msgs = mem.dev<SamplerMsgDev>(cap, false);
+        return mem.ok() && FW_CUDA(cudaEventCreateWithFlags(&ev_staged, cudaEventDisableTiming));
     }
     // cmds[0..n): the CMD_SAMPLER commands of this node for the chunk, in push order
     bool stage_sampler(const Cmd* const* cmds, uint32_t n, cudaStream_t st) {
@@ -251,7 +264,7 @@ struct NodeDeviceState {
 };
 
 struct Plan {
-    int device = 0;
+    explicit Plan(int device) : mem(device) {}
     Schedule sched;
     std::vector<std::shared_ptr<NodeDeviceState>> states;   // keeps every referenced node state alive
     std::vector<Id> nodes_to_remove;
@@ -289,15 +302,7 @@ struct Plan {
     uint16_t* d_slot_of = nullptr;             // sampler graphs: record slot per (block, voice)
     std::vector<SmpRec*> d_srec;               // per SamplerNode: [block][voice]
     std::vector<uint64_t*> d_custom_masks;     // per custom node (index = GNode::custom_idx): dense [block][voice] input masks
-    ~Plan() {
-        cudaSetDevice(device);
-        cudaFree(d_part[0]); cudaFree(d_part[1]); cudaFree(d_tmp[0]); cudaFree(d_tmp[1]); cudaFree(d_pool); cudaFree(d_slot_of);
-        for (SmpRec* q : d_srec) cudaFree(q);
-        for (uint64_t* q : d_custom_masks) cudaFree(q);
-        cudaFree(d_flags); cudaFree(rec.modes); cudaFree(rec.vals); cudaFree(rec.curves);
-        cudaFree(rec.steady_k); cudaFree(rec.gout_mask); cudaFree(rec.error); cudaFree(d_bus_mask);
-        cudaFree(rec.st_modes); cudaFree(rec.st_vals); cudaFree(rec.sum_masks); cudaFree(rec.st_sum_masks);
-    }
+    DevMem mem;  // d_flags, the records, d_bus_mask and the scratch; declared last so that it frees them before the node states go
 };
 
 // NCCL, resolved at run time with dlopen("libnccl.so.2"): no link-time dependency, and inside a process that
@@ -380,6 +385,19 @@ struct fw_processor {
     uint64_t* h_masks = nullptr; uint32_t* h_err = nullptr;  // pinned
     // optional per-kernel-class timing (CUDA events on `stream`)
     bool profiling = false; std::vector<cudaEvent_t> prof_ev; std::vector<int> prof_class; size_t prof_used = 0;
+    DevMem mem;  // I/O staging, d_flush, the bus exchange buffers, d_handover, h_masks, h_err
+    explicit fw_processor(int dev) : device(dev), mem(dev) {}
+    // Releases what the handles name; a processor that activate() only partly built has null handles for the rest.
+    ~fw_processor() {
+        cudaSetDevice(device);
+        if (side) cudaStreamDestroy(side);
+        for (cudaEvent_t e : ev_exchange_done) if (e) cudaEventDestroy(e);
+        if (nccl_comm) g_nccl.CommDestroy(nccl_comm);
+        for (cudaEvent_t e : ev) if (e) cudaEventDestroy(e);
+        for (cudaEvent_t e : prof_ev) if (e) cudaEventDestroy(e);
+        for (auto& g : graphs) if (g.exec) cudaGraphExecDestroy(g.exec);
+        if (stream) cudaStreamDestroy(stream);
+    }
 };
 
 struct ProfScope {  // brackets the launches of one kernel class with a pair of events
@@ -435,7 +453,7 @@ static bool lower(fw_ctx* c, const Schedule& s, Plan* plan, std::string* why) {
     for (size_t i = 0; i < n; ++i) {  // SamplerNodes: per-voice transport state lives in the node's device state
         if (tb.nodes[i].kind != FW_NODE_SAMPLER) continue;
         if (tb.n_samplers >= (uint32_t)kMaxSamplers) { *why = "more than 4 SamplerNodes in one voice graph"; return false; }
-        std::shared_ptr<NodeDeviceState> st = c->node_states[s.nodes[i].id.pack()];
+        const std::shared_ptr<NodeDeviceState>& st = plan->states[i];
         SamplerCtl& sc = tb.smp[tb.n_samplers];
         sc.playing = st->d_playing; sc.playhead = st->d_playhead; sc.loop_flags = st->d_loop_flags; sc.loop_start = st->d_loop_start; sc.loop_end = st->d_loop_end; sc.res = st->d_res;
         sc.n_out = (uint32_t)s.nodes[i].out.size();
@@ -445,7 +463,7 @@ static bool lower(fw_ctx* c, const Schedule& s, Plan* plan, std::string* why) {
     for (size_t i = 0; i < n; ++i) {
         if (tb.nodes[i].kind != FW_NODE_RESAMPLER) continue;
         if (tb.n_resamplers >= (uint32_t)kMaxSamplers) { *why = "more than 4 ResamplerNodes in one voice graph"; return false; }
-        std::shared_ptr<NodeDeviceState> st = c->node_states[s.nodes[i].id.pack()];
+        const std::shared_ptr<NodeDeviceState>& st = plan->states[i];
         RsCtl& rc = tb.rs[tb.n_resamplers];
         rc.flags = st->d_rs_flags; rc.res = st->d_rs_res; rc.n_out = (uint32_t)s.nodes[i].out.size();
         tb.nodes[i].sm1 = (int16_t)tb.n_resamplers++;
@@ -466,7 +484,7 @@ static bool lower(fw_ctx* c, const Schedule& s, Plan* plan, std::string* why) {
     size_t first = 1;
     if (width == 0 && n >= 3 && tb.nodes[1].kind == FW_NODE_SAMPLER && s.nodes[1].in.empty() && s.nodes[1].out.size() >= 1 && s.nodes[1].out.size() <= 2) {
         // no stream inputs: a SamplerNode heads the chain (BASELINE config 5: sampler -> gain -> pan -> ... -> bus)
-        Plan::Stage hs; hs.kind = Plan::STAGE_SAMPLER; hs.c_in = 0; hs.c_out = (uint32_t)s.nodes[1].out.size(); hs.node = c->node_states[s.nodes[1].id.pack()]; hs.sampler_sm = sm_of_node[1];
+        Plan::Stage hs; hs.kind = Plan::STAGE_SAMPLER; hs.c_in = 0; hs.c_out = (uint32_t)s.nodes[1].out.size(); hs.node = plan->states[1]; hs.sampler_sm = sm_of_node[1];
         plan->stages.push_back(hs);
         width = hs.c_out; prev = s.nodes[1].id; first = 2;
     }
@@ -490,20 +508,20 @@ static bool lower(fw_ctx* c, const Schedule& s, Plan* plan, std::string* why) {
         const uint32_t kind = nr->params->kind;
         if (kind == FW_NODE_CONV_REVERB) {
             close_pointwise(false);
-            Plan::Stage ts; ts.kind = Plan::STAGE_REVERB; ts.c_in = ts.c_out = width; ts.node = c->node_states[sn.id.pack()];
+            Plan::Stage ts; ts.kind = Plan::STAGE_REVERB; ts.c_in = ts.c_out = width; ts.node = plan->states[i];
             plan->stages.push_back(ts);
             prev = sn.id;
             continue;
         }
         if (kind == FW_NODE_SVF) {
             close_pointwise(false);
-            Plan::Stage ts; ts.kind = Plan::STAGE_TEMPORAL; ts.c_in = ts.c_out = width; ts.node = c->node_states[sn.id.pack()];
+            Plan::Stage ts; ts.kind = Plan::STAGE_TEMPORAL; ts.c_in = ts.c_out = width; ts.node = plan->states[i];
             plan->stages.push_back(ts);
             prev = sn.id;
             continue;
         }
         if (kind == FW_NODE_BIQUAD || kind == FW_NODE_DELAY) {
-            std::shared_ptr<NodeDeviceState> st = c->node_states[sn.id.pack()];
+            const std::shared_ptr<NodeDeviceState>& st = plan->states[i];
             // a delay directly after a biquad joins its pass; anything else opens a new temporal stage
             if (kind == FW_NODE_DELAY && !plan->stages.empty() && plan->stages.back().kind == Plan::STAGE_TEMPORAL && !plan->stages.back().delay &&
                 plan->stages.back().node && plan->stages.back().node->kind == FW_NODE_BIQUAD && cur.prog.n_ops == 0) {
@@ -549,7 +567,7 @@ static bool lower(fw_ctx* c, const Schedule& s, Plan* plan, std::string* why) {
         for (size_t i = 0; i < n; ++i) {
             const SchedNode& sn = s.nodes[i];
             NodeRec* nr = g.node(sn.id);
-            Plan::GNode gn; gn.kind = nr->params->kind; gn.st = c->node_states[sn.id.pack()];
+            Plan::GNode gn; gn.kind = nr->params->kind; gn.st = plan->states[i];
             for (const InAssign& a : sn.in) { gn.in_buf.push_back(a.buffer); gn.in_clear.push_back(a.should_clear); }
             for (const OutAssign& a : sn.out) gn.out_buf.push_back(a.buffer);
             gn.sm0 = sm_of_node[i]; gn.sm1 = gn.kind == FW_NODE_PAN ? sm_of_node[i] + 1 : -1;
@@ -639,7 +657,8 @@ static bool lower(fw_ctx* c, const Schedule& s, Plan* plan, std::string* why) {
     // ---- device allocations (main thread) ----
     const uint32_t V = c->cfg.num_voices, F = c->max_block_frames;
     plan->num_voices = V; plan->block_frames = F; plan->bus = c->cfg.master_bus != 0;
-    plan->d_flags = dev_alloc<uint64_t>(V);
+    DevMem& mem = plan->mem;
+    plan->d_flags = mem.dev<uint64_t>(V);
     Records& r = plan->rec;
     r.n_smoothers = n_sm;
     // Longest transient a record buffer must hold: a ramp decays like b^n with tau = smooth_secs * sample_rate samples and settles at
@@ -652,39 +671,36 @@ static bool lower(fw_ctx* c, const Schedule& s, Plan* plan, std::string* why) {
         r.kt_max = (n_sm ? ramp_blocks : 4u) + 8u * (uint32_t)plan->samplers.size();  // every sample that ends mid-call opens a short transient of its own
         r.kt_max = std::max(2u, std::min(r.kt_max, kc));
     }
-    r.modes = dev_alloc<uint32_t>((size_t)r.kt_max * V);
-    r.vals = dev_alloc<float>((size_t)r.kt_max * (n_sm ? n_sm : 1) * V);
-    r.curves = dev_alloc<float>((size_t)r.kt_max * n_sm * V * F, false);
-    r.steady_k = dev_alloc<uint32_t>(V);
-    r.gout_mask = dev_alloc<uint64_t>(V);
-    r.st_modes = dev_alloc<uint32_t>(V);
-    r.st_vals = dev_alloc<float>((size_t)(n_sm ? n_sm : 1) * V);
+    r.modes = mem.dev<uint32_t>((size_t)r.kt_max * V);
+    r.vals = mem.dev<float>((size_t)r.kt_max * (n_sm ? n_sm : 1) * V);
+    r.curves = mem.dev<float>((size_t)r.kt_max * n_sm * V * F, false);
+    r.steady_k = mem.dev<uint32_t>(V);
+    r.gout_mask = mem.dev<uint64_t>(V);
+    r.st_modes = mem.dev<uint32_t>(V);
+    r.st_vals = mem.dev<float>((size_t)(n_sm ? n_sm : 1) * V);
     r.n_sum_masks = n_sum_masks;
-    r.sum_masks = dev_alloc<uint64_t>((size_t)r.kt_max * (n_sum_masks ? n_sum_masks : 1) * V);
-    r.st_sum_masks = dev_alloc<uint64_t>((size_t)(n_sum_masks ? n_sum_masks : 1) * V);
-    r.error = dev_alloc<uint32_t>(1);
-    plan->d_bus_mask = dev_alloc<uint64_t>(1);
+    r.sum_masks = mem.dev<uint64_t>((size_t)r.kt_max * (n_sum_masks ? n_sum_masks : 1) * V);
+    r.st_sum_masks = mem.dev<uint64_t>((size_t)(n_sum_masks ? n_sum_masks : 1) * V);
+    r.error = mem.dev<uint32_t>(1);
+    plan->d_bus_mask = mem.dev<uint64_t>(1);
     {   // per-call scratch for one chunk (see Plan)
         const uint32_t Tc = c->max_call_frames, Kc = (Tc + F - 1) / F;
         plan->chunk_frames = Tc; plan->chunk_blocks = Kc;
         const uint32_t n_out = plan->c_out, groups = chain_voice_groups(V);
-        bool ok = true;
         if (plan->bus) {
-            plan->d_part[0] = dev_alloc<float>((size_t)groups * n_out * Tc, false); plan->d_part[1] = dev_alloc<float>((size_t)((groups + 15) / 16) * n_out * Tc, false);
-            ok = ok && plan->d_part[0] && plan->d_part[1];
+            plan->d_part[0] = mem.dev<float>((size_t)groups * n_out * Tc, false); plan->d_part[1] = mem.dev<float>((size_t)((groups + 15) / 16) * n_out * Tc, false);
         }
-        if (!plan->generic && plan->stages.size() > 1) { plan->d_tmp[0] = dev_alloc<float>((size_t)V * 2 * Tc, false); ok = ok && plan->d_tmp[0]; }
-        if (!plan->generic && plan->stages.size() > 2) { plan->d_tmp[1] = dev_alloc<float>((size_t)V * 2 * Tc, false); ok = ok && plan->d_tmp[1]; }
-        if (plan->generic) { plan->d_pool = dev_alloc<float>((size_t)plan->num_buffers * V * Tc, false); ok = ok && plan->d_pool; }
+        if (!plan->generic && plan->stages.size() > 1) plan->d_tmp[0] = mem.dev<float>((size_t)V * 2 * Tc, false);
+        if (!plan->generic && plan->stages.size() > 2) plan->d_tmp[1] = mem.dev<float>((size_t)V * 2 * Tc, false);
+        if (plan->generic) plan->d_pool = mem.dev<float>((size_t)plan->num_buffers * V * Tc, false);
         if (!plan->samplers.empty()) {
-            plan->d_slot_of = dev_alloc<uint16_t>((size_t)Kc * V); ok = ok && plan->d_slot_of;
-            for (size_t i = 0; i < plan->samplers.size(); ++i) { plan->d_srec.push_back(dev_alloc<SmpRec>((size_t)Kc * V)); ok = ok && plan->d_srec.back(); }
+            plan->d_slot_of = mem.dev<uint16_t>((size_t)Kc * V);
+            for (size_t i = 0; i < plan->samplers.size(); ++i) plan->d_srec.push_back(mem.dev<SmpRec>((size_t)Kc * V));
         }
-        for (auto& gn : plan->gnodes) if (gn.kind == FW_NODE_CUSTOM) { gn.custom_idx = (int)plan->d_custom_masks.size(); plan->d_custom_masks.push_back(dev_alloc<uint64_t>((size_t)Kc * V)); ok = ok && plan->d_custom_masks.back(); }
-        if (!ok) { *why = "device allocation failed: " + g_dev_err; return false; }
+        for (auto& gn : plan->gnodes) if (gn.kind == FW_NODE_CUSTOM) { gn.custom_idx = (int)plan->d_custom_masks.size(); plan->d_custom_masks.push_back(mem.dev<uint64_t>((size_t)Kc * V)); }
         r.slot_of = plan->d_slot_of;
     }
-    if (!plan->d_flags || !r.modes || !r.vals || !r.curves || !r.steady_k || !r.gout_mask || !r.error || !plan->d_bus_mask || !r.st_modes || !r.st_vals || !r.sum_masks || !r.st_sum_masks) { *why = g_dev_err; return false; }
+    if (!mem.ok()) { *why = "device allocation failed: " + g_dev_err; return false; }
     plan->tables = tb;
     {   // delay cursors, reverb history cursors + tensor maps, resampler positions and plugin calls change from call to call
         bool g = true;
@@ -719,17 +735,14 @@ static std::shared_ptr<NodeParams> params_from_desc(const fw_node_desc* d, uint3
             p->pan.assign(V, d->f0); p->gain_l.assign(V, (float)std::cos(th)); p->gain_r.assign(V, (float)std::sin(th));
             break;
         }
-        case FW_NODE_BIQUAD:
+        case FW_NODE_BIQUAD: case FW_NODE_SVF: {  // identity stages: biquad b0 = 1; SVF a1 = m0 = 1
+            const uint32_t w = coeff_width(d->kind);
             p->num_stages = d->u0 > 8 ? 8 : d->u0;
-            p->coeffs.assign((size_t)V * p->num_stages * 5, 0.0f);
-            for (size_t i = 0; i < (size_t)V * p->num_stages; ++i) p->coeffs[i * 5] = 1.0f;
+            p->coeffs.assign((size_t)V * p->num_stages * w, 0.0f);
+            for (size_t i = 0; i < (size_t)V * p->num_stages; ++i) { p->coeffs[i * w] = 1.0f; if (d->kind == FW_NODE_SVF) p->coeffs[i * w + 3] = 1.0f; }
             break;
+        }
         case FW_NODE_DELAY: p->delay = d->u0; break;
-        case FW_NODE_SVF:
-            p->num_stages = d->u0 > 8 ? 8 : d->u0;
-            p->svf_coeffs.assign((size_t)V * p->num_stages * 6, 0.0f);
-            for (size_t i = 0; i < (size_t)V * p->num_stages; ++i) { p->svf_coeffs[i * 6] = 1.0f; p->svf_coeffs[i * 6 + 3] = 1.0f; }  // identity
-            break;
         case FW_NODE_RESAMPLER:
             if (!d->data || d->u0 == 0 || d->u1 == 0 || d->data_len < (uint64_t)d->u0 * d->u1) return nullptr;
             p->rs_phases = d->u0; p->rs_taps = d->u1; p->rs_table.assign(d->data, d->data + (size_t)d->u0 * d->u1);
@@ -943,7 +956,7 @@ fw_ctx* fw_ctx_new_batched(fw_ctx* flat, int32_t device, uint32_t max_call_frame
             }
         };
         gather(&NodeParams::percent, 1); gather(&NodeParams::raw_gain, 1); gather(&NodeParams::pan, 1); gather(&NodeParams::gain_l, 1); gather(&NodeParams::gain_r, 1);
-        gather(&NodeParams::coeffs, (size_t)p->num_stages * 5); gather(&NodeParams::svf_coeffs, (size_t)p->num_stages * 6);
+        gather(&NodeParams::coeffs, (size_t)p->num_stages * coeff_width(p->kind));
         if (p->kind == FW_NODE_SAMPLER) { p->smp_active = false; p->smp_playing.assign(V, 0); p->smp_pending.assign(V, 0); p->smp_pending_epoch.assign(V, 0); }
         ids[i] = b->graph->add_node(r0.num_inputs, r0.num_outputs, std::move(p));
         if (template_ids && i < cap) template_ids[i] = ids[i].pack();
@@ -971,7 +984,7 @@ uint32_t fw_node_read_params(fw_ctx* c, fw_node_id node, uint32_t which, float* 
         case FW_PARAM_PAN: src = &p.pan; break;
         case FW_PARAM_GAIN_L: src = &p.gain_l; break;
         case FW_PARAM_GAIN_R: src = &p.gain_r; break;
-        case FW_PARAM_COEFFS: src = p.kind == FW_NODE_SVF ? &p.svf_coeffs : &p.coeffs; break;
+        case FW_PARAM_COEFFS: src = &p.coeffs; break;
         default: return 0;
     }
     for (size_t i = 0; i < src->size() && i < cap && out; ++i) out[i] = (*src)[i];
@@ -1054,19 +1067,23 @@ template <class G> static int sampler_push(fw_ctx* c, fw_node_id node, uint32_t 
 static bool gate_always(NodeParams&, uint32_t, bool) { return true; }
 extern "C" {
 void fw_ctx_set_event_block(fw_ctx* c, uint32_t block) { if (c) c->event_block = block; }
-// ---- SVF + polyphase resampler (spec ours) ----------------------------------------------------
-int fw_svf_set_coeffs(fw_ctx* c, fw_node_id node, uint32_t voice, uint32_t stage, const float* k) {
-    NodeParams* p = params_of(c, node, FW_NODE_SVF);
+// ---- biquad / SVF coefficient table: [voice][stage][coeff_width(kind)] ------------------------
+static int set_stage_coeffs(fw_ctx* c, fw_node_id node, uint32_t kind, uint32_t voice, uint32_t stage, const float* k) {
+    NodeParams* p = params_of(c, node, kind);
     if (!p || !k || stage >= p->num_stages) return -1;
-    Cmd m{}; m.kind = CMD_SVF; m.a = stage; std::memcpy(m.f, k, 6 * sizeof(float));
-    return store_param(c, p, voice, m, [&](uint32_t v) { std::memcpy(&p->svf_coeffs[((size_t)v * p->num_stages + stage) * 6], k, 6 * sizeof(float)); });
+    const uint32_t w = coeff_width(kind);
+    Cmd m{}; m.kind = CMD_COEFFS; m.a = stage; std::memcpy(m.f, k, w * sizeof(float));
+    return store_param(c, p, voice, m, [&](uint32_t v) { std::memcpy(&p->coeffs[((size_t)v * p->num_stages + stage) * w], k, w * sizeof(float)); });
 }
-int fw_svf_set_all_coeffs(fw_ctx* c, fw_node_id node, const float* k, uint32_t nv, uint32_t ns) {
-    NodeParams* p = params_of(c, node, FW_NODE_SVF);
+static int set_all_coeffs(fw_ctx* c, fw_node_id node, uint32_t kind, const float* k, uint32_t nv, uint32_t ns) {
+    NodeParams* p = params_of(c, node, kind);
     if (!p || !k || nv != p->num_voices || ns != p->num_stages) return -1;
-    std::memcpy(p->svf_coeffs.data(), k, (size_t)nv * ns * 6 * sizeof(float));
-    return upload_array(c, p, 2, p->svf_coeffs.data(), p->svf_coeffs.size());
+    std::memcpy(p->coeffs.data(), k, (size_t)nv * ns * coeff_width(kind) * sizeof(float));
+    return upload_array(c, p, 2, p->coeffs.data(), p->coeffs.size());
 }
+// ---- SVF + polyphase resampler (spec ours) ----------------------------------------------------
+int fw_svf_set_coeffs(fw_ctx* c, fw_node_id node, uint32_t voice, uint32_t stage, const float* k) { return set_stage_coeffs(c, node, FW_NODE_SVF, voice, stage, k); }
+int fw_svf_set_all_coeffs(fw_ctx* c, fw_node_id node, const float* k, uint32_t nv, uint32_t ns) { return set_all_coeffs(c, node, FW_NODE_SVF, k, nv, ns); }
 void fw_svf_design(uint32_t type, double fc, double q, double sr, float* out) {
     const double g = std::tan(M_PI * fc / sr), k = 1.0 / q;
     const double a1 = 1.0 / (1.0 + g * (g + k)), a2 = g * a1, a3 = g * a2;
@@ -1109,7 +1126,7 @@ void fw_resampler_design(uint32_t P, uint32_t T, double cutoff, double beta, flo
 // ---- sample resources + SamplerNode (sampler.rs:46-181) --------------------------------------
 uint32_t fw_sample_resource_create(fw_ctx* c, uint32_t format, uint32_t channels, uint64_t frames, const void* data) {
     if (!c || !data || format > FW_SAMPLE_U16_PLANAR || channels == 0 || channels > 64 || frames == 0) return 0;
-    if (!c->res) { c->res = std::make_shared<ResTable>(); c->res->device = c->cfg.device; }
+    if (!c->res) c->res = std::make_shared<ResTable>(c->cfg.device);
     return c->res->add(format, channels, frames, data);
 }
 int fw_sampler_set_sample(fw_ctx* c, fw_node_id node, uint32_t voice, uint32_t res, int stop_playback) {
@@ -1186,18 +1203,8 @@ int fw_pan_set_pans(fw_ctx* c, fw_node_id node, const float* pan, uint32_t n) {
     return r0 ? r0 : r1;
 }
 int fw_pan_set_gains(fw_ctx* c, fw_node_id node, uint32_t voice, float gl, float gr) { return set_pan_gains(c, params_of(c, node, FW_NODE_PAN), voice, gl, gr, nullptr); }
-int fw_biquad_set_coeffs(fw_ctx* c, fw_node_id node, uint32_t voice, uint32_t stage, const float* k) {
-    NodeParams* p = params_of(c, node, FW_NODE_BIQUAD);
-    if (!p || !k || stage >= p->num_stages) return -1;
-    Cmd m{}; m.kind = CMD_BIQUAD; m.a = stage; std::memcpy(m.f, k, 5 * sizeof(float));
-    return store_param(c, p, voice, m, [&](uint32_t v) { std::memcpy(&p->coeffs[((size_t)v * p->num_stages + stage) * 5], k, 5 * sizeof(float)); });
-}
-int fw_biquad_set_all_coeffs(fw_ctx* c, fw_node_id node, const float* k, uint32_t nv, uint32_t ns) {
-    NodeParams* p = params_of(c, node, FW_NODE_BIQUAD);
-    if (!p || !k || nv != p->num_voices || ns != p->num_stages) return -1;
-    std::memcpy(p->coeffs.data(), k, (size_t)nv * ns * 5 * sizeof(float));
-    return upload_array(c, p, 2, p->coeffs.data(), p->coeffs.size());
-}
+int fw_biquad_set_coeffs(fw_ctx* c, fw_node_id node, uint32_t voice, uint32_t stage, const float* k) { return set_stage_coeffs(c, node, FW_NODE_BIQUAD, voice, stage, k); }
+int fw_biquad_set_all_coeffs(fw_ctx* c, fw_node_id node, const float* k, uint32_t nv, uint32_t ns) { return set_all_coeffs(c, node, FW_NODE_BIQUAD, k, nv, ns); }
 void fw_biquad_design_rbj(uint32_t type, double fc, double q, double gain_db, double sr, float* out) {  // RBJ cookbook, f64 -> f32
     const double w0 = 2.0 * M_PI * fc / sr, cw = std::cos(w0), sw = std::sin(w0), alpha = sw / (2.0 * q), A = std::pow(10.0, gain_db / 40.0);
     double b0, b1, b2, a0, a1, a2;
@@ -1227,29 +1234,27 @@ int fw_ctx_activate(fw_ctx* c, uint32_t sr, uint32_t n_in, uint32_t n_out, uint3
         return -1;
     }
     if (!FW_CUDA(cudaSetDevice(c->cfg.device))) { c->last_error = g_dev_err; return -1; }
-    auto* p = new fw_processor();
-    p->device = c->cfg.device;
+    auto p = std::make_unique<fw_processor>(c->cfg.device);  // the context turns active only once the processor is complete
     bool ok = FW_CUDA(cudaStreamCreateWithFlags(&p->stream, cudaStreamNonBlocking));
     for (int i = 0; ok && i < 4; ++i) ok = FW_CUDA(cudaEventCreate(&p->ev[i]));
-    ok = ok && FW_CUDA(cudaMallocHost(&p->h_masks, sizeof(uint64_t) * (c->cfg.num_voices + 1))) && FW_CUDA(cudaMallocHost(&p->h_err, sizeof(uint32_t)));
-    if (!ok) { c->last_error = g_dev_err; delete p; return -1; }
-    c->ch = std::make_shared<Channels>(std::max<size_t>(4096, 4 * (size_t)c->cfg.num_voices));
-    c->active = true; c->sample_rate = sr; c->max_block_frames = mbf; c->n_in = n_in; c->n_out = n_out;
-    p->ch = c->ch; p->user_cx = user_cx; p->num_voices = c->cfg.num_voices; p->max_block_frames = mbf; p->n_in = n_in; p->n_out = n_out;
+    p->h_masks = p->mem.host<uint64_t>(c->cfg.num_voices + 1); p->h_err = p->mem.host<uint32_t>(1);
+    if (!ok || !p->mem.ok()) { c->last_error = g_dev_err; return -1; }
     p->bus = c->cfg.master_bus != 0;
-    c->max_call_frames = c->cfg.max_call_frames ? c->cfg.max_call_frames : 64u * mbf;
-    c->max_call_frames = ((c->max_call_frames + mbf - 1) / mbf) * mbf;  // whole blocks
-    p->max_call_frames = c->max_call_frames;
-    p->pend.resize(2 * c->ch->cmds.capacity()); p->cmd_ptrs.resize(p->pend.size());
+    const uint32_t max_call = c->cfg.max_call_frames ? c->cfg.max_call_frames : 64u * mbf;
+    p->max_call_frames = ((max_call + mbf - 1) / mbf) * mbf;  // whole blocks
     {
         const size_t V = c->cfg.num_voices, Tm = p->max_call_frames;
         const size_t in_e = V * n_in * Tm, out_e = (size_t)(p->bus ? 1 : V) * n_out * Tm;
-        p->d_in = dev_alloc<float>(in_e, false); p->d_out = dev_alloc<float>(out_e, false); p->d_inter = dev_alloc<float>(std::max(in_e, out_e), false);
-        if (!p->d_in || !p->d_out || !p->d_inter) { c->last_error = "device allocation failed (I/O staging for max_call_frames): " + g_dev_err; cudaFree(p->d_in); cudaFree(p->d_out); cudaFree(p->d_inter); delete p; c->active = false; c->ch.reset(); return -1; }
+        p->d_in = p->mem.dev<float>(in_e, false); p->d_out = p->mem.dev<float>(out_e, false); p->d_inter = p->mem.dev<float>(std::max(in_e, out_e), false);
+        if (!p->mem.ok()) { c->last_error = "device allocation failed (I/O staging for max_call_frames): " + g_dev_err; return -1; }
     }
+    c->ch = std::make_shared<Channels>(std::max<size_t>(4096, 4 * (size_t)c->cfg.num_voices));
+    c->active = true; c->sample_rate = sr; c->max_block_frames = mbf; c->n_in = n_in; c->n_out = n_out; c->max_call_frames = p->max_call_frames;
+    p->ch = c->ch; p->user_cx = user_cx; p->num_voices = c->cfg.num_voices; p->max_block_frames = mbf; p->n_in = n_in; p->n_out = n_out;
+    p->pend.resize(2 * c->ch->cmds.capacity()); p->cmd_ptrs.resize(p->pend.size());
     // SmootherConfig::default + ParamSmoother::new (smoother.rs:18-25,99-100); host libm, once
     p->sm_b = std::exp(-1.0f / ((10.0f / 1000.0f) * (float)sr)); p->sm_a = 1.0f - p->sm_b; p->sm_eps = 0.00001f;
-    *out = p;
+    *out = p.release();
     return 0;
 }
 int fw_ctx_is_activated(fw_ctx* c) { return c->active; }
@@ -1268,8 +1273,7 @@ int fw_ctx_update(fw_ctx* c, fw_update_status* out) {  // context.rs:93-148
     st.kind = FW_UPDATE_ACTIVE;
     if (!c->graph->needs_compile()) return done();
     cudaSetDevice(c->cfg.device);
-    auto plan = std::make_unique<Plan>();
-    plan->device = c->cfg.device;
+    auto plan = std::make_unique<Plan>(c->cfg.device);
     CompileError e = c->graph->compile_schedule(c->max_block_frames, &plan->sched);
     if (e.code != FW_COMPILE_OK) { st.graph_error = e.code; st.error_node = e.node.pack(); st.error_port = e.port; return done(); }
     // A live node whose port count changed (set_num_inputs / set_num_outputs, graph.rs:315-393) no longer matches the per-channel
@@ -1292,8 +1296,8 @@ int fw_ctx_update(fw_ctx* c, fw_update_status* out) {  // context.rs:93-148
         std::string msg = node_check_activation(*r->params, r->num_inputs, r->num_outputs);
         std::shared_ptr<NodeDeviceState> ds;
         if (msg.empty()) {
-            ds = std::make_shared<NodeDeviceState>();
-            ds->device = c->cfg.device; ds->kind = r->params->kind; ds->V = c->cfg.num_voices; ds->params = r->params; ds->channels = r->num_inputs;
+            ds = std::make_shared<NodeDeviceState>(c->cfg.device);
+            ds->kind = r->params->kind; ds->V = c->cfg.num_voices; ds->params = r->params; ds->channels = r->num_inputs;
             if (r->params->custom) {  // AudioNode::activate (node.rs:12-18)
                 char err[256] = {0};
                 void* proc_h = nullptr;
@@ -1304,7 +1308,7 @@ int fw_ctx_update(fw_ctx* c, fw_update_status* out) {  // context.rs:93-148
                     ds->custom_proc = proc_h;
                 }
             }
-            if (ds->kind == FW_NODE_SAMPLER || ds->kind == FW_NODE_RESAMPLER) { if (!c->res) { c->res = std::make_shared<ResTable>(); c->res->device = c->cfg.device; } ds->res_table = c->res; }
+            if (ds->kind == FW_NODE_SAMPLER || ds->kind == FW_NODE_RESAMPLER) { if (!c->res) c->res = std::make_shared<ResTable>(c->cfg.device); ds->res_table = c->res; }
             if (!ds->create()) msg = "device allocation failed: " + g_dev_err;
         }
         if (!msg.empty()) {
@@ -1705,8 +1709,8 @@ static bool apply_commands(fw_processor* p, Plan& pl, uint32_t b) {
         if (m.kind == CMD_UPLOAD) {  // ring order: earlier single stores are flushed first, later ones come after this copy
             float* snap = reinterpret_cast<float*>(m.x);
             if (st) {
-                float* dst = m.a < 2 ? (m.a < st->n_sm ? st->d_target[m.a] : nullptr) : ((st->kind == FW_NODE_BIQUAD || st->kind == FW_NODE_SVF) ? st->d_coeffs : nullptr);
-                const size_t cap = m.a < 2 ? (size_t)V : (size_t)V * st->params->num_stages * (st->kind == FW_NODE_SVF ? 6 : 5);
+                float* dst = m.a < 2 ? (m.a < st->n_sm ? st->d_target[m.a] : nullptr) : (coeff_width(st->kind) ? st->d_coeffs : nullptr);
+                const size_t cap = m.a < 2 ? (size_t)V : (size_t)V * st->params->num_stages * coeff_width(st->kind);
                 pk.flush();
                 if (dst && m.y <= cap) pk.ok = pk.ok && FW_CUDA(cudaMemcpyAsync(dst, snap, m.y * sizeof(float), cudaMemcpyHostToDevice, p->stream));  // pageable source: staged before the call returns
             }
@@ -1717,8 +1721,11 @@ static bool apply_commands(fw_processor* p, Plan& pl, uint32_t b) {
         const uint32_t cnt = m.voice == FW_ALL_VOICES ? V : 1u; const size_t v0 = m.voice == FW_ALL_VOICES ? 0 : m.voice;
         switch (m.kind) {
             case CMD_TARGET: if (m.a < st->n_sm) pk.f32(st->d_target[m.a], m.voice, V, 1, 0, m.f[0]); break;
-            case CMD_BIQUAD: if (st->kind == FW_NODE_BIQUAD && m.a < st->params->num_stages) for (int k = 0; k < 5; ++k) pk.f32(st->d_coeffs, m.voice, V, (size_t)st->params->num_stages * 5, (size_t)m.a * 5 + k, m.f[k]); break;
-            case CMD_SVF: if (st->kind == FW_NODE_SVF && m.a < st->params->num_stages) for (int k = 0; k < 6; ++k) pk.f32(st->d_coeffs, m.voice, V, (size_t)st->params->num_stages * 6, (size_t)m.a * 6 + k, m.f[k]); break;
+            case CMD_COEFFS: {
+                const uint32_t w = coeff_width(st->kind), ns = st->params->num_stages;
+                if (w && m.a < ns) for (uint32_t k = 0; k < w; ++k) pk.f32(st->d_coeffs, m.voice, V, (size_t)ns * w, (size_t)m.a * w + k, m.f[k]);
+                break;
+            }
             case CMD_RS_SET:
                 if (st->kind != FW_NODE_RESAMPLER) break;
                 pk.add(st->d_rs_res + v0, m.b, 4, cnt, 4); pk.add(st->d_rs_flags + v0, m.a, 4, cnt, 4); pk.add(st->d_rs_step + v0, m.x, 8, cnt, 8);
@@ -2008,17 +2015,10 @@ void fw_processor_free(fw_processor* p) {  // Drop processor.rs:251-263
     cudaSetDevice(p->device);
     join_side(p);
     cudaStreamSynchronize(p->stream);
-    if (p->side) { cudaStreamSynchronize(p->side); cudaStreamDestroy(p->side); cudaEventDestroy(p->ev_exchange_done[0]); cudaEventDestroy(p->ev_exchange_done[1]); }
+    if (p->side) cudaStreamSynchronize(p->side);
     ProcToCtx m; m.kind = 1; m.plan = p->plan; m.user_cx = p->user_cx;
     if (!p->ch->to_ctx.push(m)) delete p->plan;
-    cudaFree(p->d_in); cudaFree(p->d_out); cudaFree(p->d_inter); cudaFree(p->d_flush); cudaFree(p->d_bus_local[0]); cudaFree(p->d_bus_local[1]); cudaFree(p->d_gather[0]); cudaFree(p->d_gather[1]); cudaFree(p->d_handover);
-    if (p->nccl_comm) g_nccl.CommDestroy(p->nccl_comm);
-    cudaFreeHost(p->h_masks); cudaFreeHost(p->h_err);
-    for (auto& e : p->ev) if (e) cudaEventDestroy(e);
-    for (auto& e : p->prof_ev) if (e) cudaEventDestroy(e);
-    for (auto& g : p->graphs) if (g.exec) cudaGraphExecDestroy(g.exec);
     for (size_t i = 0; i < p->pend_n; ++i) if (p->pend[i].kind == CMD_UPLOAD) delete[] reinterpret_cast<float*>(p->pend[i].x);
-    cudaStreamDestroy(p->stream);
     delete p;
 }
 
@@ -2076,7 +2076,7 @@ int fw_processor_profile_read(fw_processor* p, double* ms4, uint64_t* n4) {
 int fw_processor_l2_flush(fw_processor* p) {
     cudaSetDevice(p->device);
     const size_t n = (size_t)64 << 20;  // 256 MiB of f32 > 50 MB L2
-    if (!p->d_flush) { void* q = nullptr; if (!FW_CUDA(cudaMalloc(&q, n * 4))) return -1; p->d_flush = static_cast<float*>(q); }
+    if (!p->d_flush && !(p->d_flush = p->mem.dev<float>(n, false))) return -1;
     if (!FW_CUDA(launch_fill(p->d_flush, n, 1.0f, p->stream))) return -1;
     return 0;
 }
@@ -2181,11 +2181,10 @@ int fw_processor_comm_init(fw_processor* p, int rank, int world, const uint8_t* 
         !FW_CUDA(cudaEventCreateWithFlags(&p->ev_exchange_done[1], cudaEventDisableTiming))) return -1;
     p->rank = rank; p->world = world;
     for (int q = 0; q < 2; ++q) {
-        p->d_bus_local[q] = dev_alloc<float>((size_t)p->n_out * p->max_call_frames, false); p->d_gather[q] = dev_alloc<float>((size_t)world * p->n_out * p->max_call_frames, false);
-        if (!p->d_bus_local[q] || !p->d_gather[q]) return -1;
+        p->d_bus_local[q] = p->mem.dev<float>((size_t)p->n_out * p->max_call_frames, false); p->d_gather[q] = p->mem.dev<float>((size_t)world * p->n_out * p->max_call_frames, false);
     }
-    p->d_handover = dev_alloc<uint32_t>(2);  // [0] epoch word, [1] last-CTA counter of the signalling combine
-    return p->d_handover ? 0 : -1;
+    p->d_handover = p->mem.dev<uint32_t>(2);  // [0] epoch word, [1] last-CTA counter of the signalling combine
+    return p->mem.ok() ? 0 : -1;
 }
 // Host-buffer all-gather over the processor's communicator: what a torch-free driver needs for barriers, max-over-ranks
 // timing and result cross-checks (bench.py, tests/multigpu_worker.py). Not on the audio path.
