@@ -276,15 +276,15 @@ struct Plan {
                    std::shared_ptr<NodeDeviceState> node, delay; int sampler_sm = -1; };
     std::vector<Stage> stages;
     // generic lowering (arbitrary DAG of built-in nodes): one launch group per scheduled node over pool buffers [buffer][V][T]
-    struct GNode { uint32_t kind = 0; std::vector<uint32_t> in_buf, out_buf; std::vector<uint8_t> in_clear; int sm0 = -1, sm1 = -1, mask_slot = -1, custom_idx = -1, sampler_idx = -1;
-                   float f0 = 0.0f; std::shared_ptr<NodeDeviceState> st;
-                   // fusion of pointwise runs and graph_in aliasing (see fuse_generic): a run of stereo Volume / Pan nodes, optionally ending in
-                   // graph_out, is ONE chain program launched at its last node; the others are `absorbed`. `run_in` = pool buffers the run
-                   // starts from (empty: in_buf), `pre_ops` = the ops of the absorbed nodes. `src_port` non-empty: the node (or its run) reads
-                   // the caller's input channels src_port[k] directly instead of graph_in's pool copy.
-                   bool absorbed = false; std::vector<ChainOp> pre_ops; std::vector<uint32_t> run_in, src_port; };
+    struct GNode { uint32_t kind = 0; std::vector<uint32_t> in_buf, out_buf; std::vector<uint8_t> in_clear; int sm0 = -1, mask_slot = -1, custom_idx = -1, sampler_idx = -1;
+                   std::shared_ptr<NodeDeviceState> st;
+                   // graph_in, graph_out and pointwise nodes launch `prog`, once or (`pairs`) per channel pair, an odd last channel narrowed
+                   // to 1 -> 1. Fusion and graph_in aliasing (see fuse_generic): a run of stereo Volume / Pan nodes, optionally ending in
+                   // graph_out, is ONE program launched at its last node, which then reads the run's first inputs (in_buf); the others are
+                   // `absorbed`, and so is graph_in when no node reads its pool copy. `src_port` non-empty: the node (or its run) reads the
+                   // caller's input channels src_port[k] instead of pool buffers.
+                   ChainProgram prog{}; bool pairs = false, absorbed = false; std::vector<uint32_t> src_port; };
     bool generic = false; std::vector<GNode> gnodes; uint32_t num_buffers = 0;
-    bool gin_copy = true;  // false: every consumer of graph_in reads the caller's buffer itself, the pool copy is skipped
     bool reads_caller_rows = false;  // some node reads the caller's input rows directly (row pitch n_in * frames must fit 32 bits)
     std::vector<std::shared_ptr<NodeDeviceState>> samplers;  // index = CtlTables::smp index
     std::vector<std::shared_ptr<NodeDeviceState>> resamplers;  // index = CtlTables::rs index
@@ -416,15 +416,30 @@ struct ProfScope {  // brackets the launches of one kernel class with a pair of 
 // =============================================================================================
 // lowering: schedule -> control tables + fused chain program
 // =============================================================================================
-static bool lower(fw_ctx* c, const Schedule& s, Plan* plan, std::string* why) {
+// The chain op of a pointwise node kind; false for every other kind. sm0: the node's first smoother; threshold_gain: HardClip's threshold.
+static bool chain_op(uint32_t kind, int sm0, float threshold_gain, ChainOp* op) {
+    *op = ChainOp{}; op->sm0 = op->sm1 = -1;
+    switch (kind) {
+        case FW_NODE_VOLUME: op->kind = OP_GAIN; op->sm0 = sm0; return true;
+        case FW_NODE_PAN: op->kind = OP_PAN; op->sm0 = sm0; op->sm1 = sm0 + 1; return true;
+        case FW_NODE_HARD_CLIP: op->kind = OP_CLIP; op->f0 = threshold_gain; return true;
+        case FW_NODE_MONO_TO_STEREO: op->kind = OP_M2S; return true;
+        case FW_NODE_STEREO_TO_MONO: op->kind = OP_S2M; return true;
+        default: return false;
+    }
+}
+
+// Control tables (one CtlNode per scheduled node, the smoothers, the sampler and resampler transport state) and the node states of
+// the plan. sm_of_node[i]: the first smoother of node i, -1: none.
+static bool lower_control(fw_ctx* c, const Schedule& s, Plan* plan, std::vector<int>* sm_of_node, std::string* why) {
     Graph& g = *c->graph;
     const size_t n = s.nodes.size();
     if (n < 2 || n > (size_t)kMaxCtlNodes) { *why = "schedule too long for the device control tables"; return false; }
     if (s.num_buffers > 64) { *why = "more than 64 buffers in one voice graph"; return false; }
-    CtlTables tb{};
+    CtlTables& tb = plan->tables;
     tb.n_nodes = (uint32_t)n; tb.n_buffers = s.num_buffers;
     uint32_t off_in = 0, off_out = 0, n_sm = 0;
-    std::vector<int> sm_of_node(n, -1);
+    sm_of_node->assign(n, -1);
     for (size_t i = 0; i < n; ++i) {
         const SchedNode& sn = s.nodes[i];
         NodeRec* nr = g.node(sn.id);
@@ -441,7 +456,7 @@ static bool lower(fw_ctx* c, const Schedule& s, Plan* plan, std::string* why) {
         plan->states.push_back(st);
         if (st->n_sm) {
             if (n_sm + st->n_sm > (uint32_t)kMaxSmoothers) { *why = "more than 16 smoothed parameters in one voice graph"; return false; }
-            sm_of_node[i] = (int)n_sm;
+            (*sm_of_node)[i] = (int)n_sm;
             cn.sm0 = (int16_t)n_sm; if (st->n_sm == 2) cn.sm1 = (int16_t)(n_sm + 1);
             for (uint32_t k = 0; k < st->n_sm; ++k) {
                 tb.sm_input[n_sm] = st->sm_input[k]; tb.sm_last[n_sm] = st->sm_last[k]; tb.sm_status[n_sm] = st->sm_status[k]; tb.sm_target[n_sm] = st->d_target[k];
@@ -449,7 +464,7 @@ static bool lower(fw_ctx* c, const Schedule& s, Plan* plan, std::string* why) {
             }
         }
     }
-    tb.n_smoothers = n_sm;
+    tb.n_smoothers = n_sm; plan->n_sm = n_sm;
     for (size_t i = 0; i < n; ++i) {  // SamplerNodes: per-voice transport state lives in the node's device state
         if (tb.nodes[i].kind != FW_NODE_SAMPLER) continue;
         if (tb.n_samplers >= (uint32_t)kMaxSamplers) { *why = "more than 4 SamplerNodes in one voice graph"; return false; }
@@ -469,20 +484,19 @@ static bool lower(fw_ctx* c, const Schedule& s, Plan* plan, std::string* why) {
         tb.nodes[i].sm1 = (int16_t)tb.n_resamplers++;
         plan->resamplers.push_back(st);
     }
-    uint32_t n_sum_masks = 0;  // generic lowering only: nodes whose data-plane body needs the per-block input silence mask
+    return true;
+}
 
+// Data plane, first choice: a linear chain graph_in -> n1 -> ... -> nk -> graph_out, port i to port i, fused into stages. False, with
+// the reason, for any other schedule.
+static bool lower_chain(const Schedule& s, const std::vector<int>& sm_of_node, bool bus, Plan* plan, std::string* why) {
+    const size_t n = s.nodes.size();
     const SchedNode& gin = s.nodes.front();
     const SchedNode& gout = s.nodes.back();
-    if (gin.out.size() != c->n_in) { *why = "stream input channels must equal the graph_in port count on the device path"; return false; }
-    if (gout.in.size() != c->n_out) { *why = "stream output channels must equal the graph_out port count on the device path"; return false; }
-    plan->c_in = (uint32_t)gin.out.size(); plan->c_out = (uint32_t)gout.in.size();
-
-    // ---- data plane, first choice: a linear chain graph_in -> n1 -> ... -> nk -> graph_out, port i to port i, fused into stages ----
-    auto chain_lower = [&]() -> bool {
     uint32_t width = (uint32_t)gin.out.size();
     Id prev = gin.id;
     size_t first = 1;
-    if (width == 0 && n >= 3 && tb.nodes[1].kind == FW_NODE_SAMPLER && s.nodes[1].in.empty() && s.nodes[1].out.size() >= 1 && s.nodes[1].out.size() <= 2) {
+    if (width == 0 && n >= 3 && plan->tables.nodes[1].kind == FW_NODE_SAMPLER && s.nodes[1].in.empty() && s.nodes[1].out.size() >= 1 && s.nodes[1].out.size() <= 2) {
         // no stream inputs: a SamplerNode heads the chain (BASELINE config 5: sampler -> gain -> pan -> ... -> bus)
         Plan::Stage hs; hs.kind = Plan::STAGE_SAMPLER; hs.c_in = 0; hs.c_out = (uint32_t)s.nodes[1].out.size(); hs.node = plan->states[1]; hs.sampler_sm = sm_of_node[1];
         plan->stages.push_back(hs);
@@ -502,10 +516,10 @@ static bool lower(fw_ctx* c, const Schedule& s, Plan* plan, std::string* why) {
     };
     for (size_t i = first; i + 1 < n; ++i) {
         const SchedNode& sn = s.nodes[i];
-        NodeRec* nr = g.node(sn.id);
+        const NodeParams& np = *plan->states[i]->params;
         if (!fed_by_prev(sn, width)) { *why = "voice graph is not a linear port-to-port chain"; return false; }
         if (sn.out.size() < 1 || sn.out.size() > 2) { *why = "the fused chain supports 1 or 2 channels"; return false; }
-        const uint32_t kind = nr->params->kind;
+        const uint32_t kind = np.kind;
         if (kind == FW_NODE_CONV_REVERB) {
             close_pointwise(false);
             Plan::Stage ts; ts.kind = Plan::STAGE_REVERB; ts.c_in = ts.c_out = width; ts.node = plan->states[i];
@@ -536,126 +550,137 @@ static bool lower(fw_ctx* c, const Schedule& s, Plan* plan, std::string* why) {
             continue;
         }
         if (cur.prog.n_ops >= (uint32_t)kMaxChainOps) { *why = "more than 16 pointwise nodes in a row"; return false; }
-        ChainOp op{}; op.sm0 = op.sm1 = -1;
-        switch (kind) {
-            case FW_NODE_VOLUME: op.kind = OP_GAIN; op.sm0 = sm_of_node[i]; break;
-            case FW_NODE_PAN: op.kind = OP_PAN; op.sm0 = sm_of_node[i]; op.sm1 = sm_of_node[i] + 1; break;
-            case FW_NODE_HARD_CLIP: op.kind = OP_CLIP; op.f0 = nr->params->threshold_gain; break;
-            case FW_NODE_MONO_TO_STEREO: op.kind = OP_M2S; break;
-            case FW_NODE_STEREO_TO_MONO: op.kind = OP_S2M; break;
-            case FW_NODE_SUM:
-                if (sn.in.size() == sn.out.size()) { prev = sn.id; continue; }  // 1-port sum == copy (sum.rs:58-65): no data op
-                *why = "SumNode with more than one port inside a voice chain"; return false;
-            default: *why = std::string("node kind '") + node_debug_name(kind) + "' has no device lowering yet"; return false;
+        if (kind == FW_NODE_SUM) {
+            if (sn.in.size() == sn.out.size()) { prev = sn.id; continue; }  // 1-port sum == copy (sum.rs:58-65): no data op
+            *why = "SumNode with more than one port inside a voice chain"; return false;
         }
+        ChainOp op;
+        if (!chain_op(kind, sm_of_node[i], np.threshold_gain, &op)) { *why = std::string("node kind '") + node_debug_name(kind) + "' has no device lowering yet"; return false; }
         cur.prog.ops[cur.prog.n_ops++] = op;
         width = (uint32_t)sn.out.size();
         prev = sn.id;
     }
     if (!fed_by_prev(gout, width)) { *why = "graph_out is not fed port-to-port by the end of the chain"; return false; }
     // the last stage must be pointwise when the master bus follows it, and a plan is never empty
-    const bool bus = c->cfg.master_bus != 0;
     close_pointwise(plan->stages.empty() || (bus && cur.prog.n_ops == 0 && plan->stages.back().kind != Plan::STAGE_POINTWISE));
     plan->c_out = width;
     return true;
-    };  // chain_lower
+}
 
-    // ---- data plane, general case: the reference's own buffer assignment on device, one launch group per scheduled node ----
-    auto generic_lower = [&]() -> bool {
-        plan->stages.clear(); plan->generic = true; plan->num_buffers = s.num_buffers;
-        if (c->cfg.master_bus && gout.in.size() > 2) { *why = "master bus over more than 2 graph_out channels"; return false; }
-        for (size_t i = 0; i < n; ++i) {
-            const SchedNode& sn = s.nodes[i];
-            NodeRec* nr = g.node(sn.id);
-            Plan::GNode gn; gn.kind = nr->params->kind; gn.st = plan->states[i];
-            for (const InAssign& a : sn.in) { gn.in_buf.push_back(a.buffer); gn.in_clear.push_back(a.should_clear); }
-            for (const OutAssign& a : sn.out) gn.out_buf.push_back(a.buffer);
-            gn.sm0 = sm_of_node[i]; gn.sm1 = gn.kind == FW_NODE_PAN ? sm_of_node[i] + 1 : -1;
-            if (gn.kind == FW_NODE_SAMPLER) gn.sampler_idx = tb.nodes[i].sm1;
-            gn.f0 = nr->params->threshold_gain;
-            const bool endpoint = i == 0 || i + 1 == n;
-            // bodies that branch on the input silence mask (see silence_fix_kernel / sum_kernel)
-            const bool needs_mask = !endpoint && ((gn.kind == FW_NODE_CUSTOM) || (!sn.out.empty() &&
-                ((gn.kind == FW_NODE_SUM && sn.in.size() != sn.out.size()) || gn.kind == FW_NODE_HARD_CLIP || (gn.kind == FW_NODE_VOLUME && sn.in.size() != 2) ||
-                 gn.kind == FW_NODE_MONO_TO_STEREO || gn.kind == FW_NODE_STEREO_TO_MONO)));
-            if (gn.kind == FW_NODE_CUSTOM && !nr->params->custom->vt.process_device) { *why = std::string("custom node '") + nr->params->custom->debug_name + "' has no process_device: it cannot run on the device (there is no CPU fallback)"; return false; }
-            if (needs_mask) {
-                if (n_sum_masks >= (uint32_t)kMaxSumMasks) { *why = "more than 32 mask-dependent nodes in one voice graph"; return false; }
-                gn.mask_slot = (int)n_sum_masks; tb.nodes[i].mask_slot = (uint8_t)(++n_sum_masks);
-            }
-            if (gn.kind == FW_NODE_DUMMY && !endpoint && !sn.out.empty()) { *why = "a DummyAudioNode inside the graph leaves its outputs stale in the reference (dummy.rs:34-41): not reproducible on the device"; return false; }
-            if (gn.kind == FW_NODE_MONO_TO_STEREO && (sn.in.size() != 1 || sn.out.size() != 2)) { *why = "MonoToStereoNode must be 1 -> 2"; return false; }
-            if (gn.kind == FW_NODE_STEREO_TO_MONO && (sn.in.size() != 2 || sn.out.size() != 1)) { *why = "StereoToMonoNode must be 2 -> 1"; return false; }
-            plan->gnodes.push_back(std::move(gn));
+// Data plane, general case: the reference's own buffer assignment on device, one launch group per scheduled node. graph_in, graph_out
+// and the pointwise nodes get the chain program they launch.
+static bool lower_generic(const Schedule& s, const std::vector<int>& sm_of_node, bool bus, Plan* plan, std::string* why) {
+    const size_t n = s.nodes.size();
+    plan->stages.clear(); plan->generic = true; plan->num_buffers = s.num_buffers;
+    if (bus && s.nodes.back().in.size() > 2) { *why = "master bus over more than 2 graph_out channels"; return false; }
+    uint32_t n_sum_masks = 0;  // nodes whose data-plane body needs the per-block input silence mask
+    for (size_t i = 0; i < n; ++i) {
+        const SchedNode& sn = s.nodes[i];
+        const NodeParams& np = *plan->states[i]->params;
+        Plan::GNode gn; gn.kind = np.kind; gn.st = plan->states[i];
+        for (const InAssign& a : sn.in) { gn.in_buf.push_back(a.buffer); gn.in_clear.push_back(a.should_clear); }
+        for (const OutAssign& a : sn.out) gn.out_buf.push_back(a.buffer);
+        gn.sm0 = sm_of_node[i];
+        if (gn.kind == FW_NODE_SAMPLER) gn.sampler_idx = plan->tables.nodes[i].sm1;
+        const bool endpoint = i == 0 || i + 1 == n;
+        // bodies that branch on the input silence mask (see silence_fix_kernel / sum_kernel)
+        const bool needs_mask = !endpoint && ((gn.kind == FW_NODE_CUSTOM) || (!sn.out.empty() &&
+            ((gn.kind == FW_NODE_SUM && sn.in.size() != sn.out.size()) || gn.kind == FW_NODE_HARD_CLIP || (gn.kind == FW_NODE_VOLUME && sn.in.size() != 2) ||
+             gn.kind == FW_NODE_MONO_TO_STEREO || gn.kind == FW_NODE_STEREO_TO_MONO)));
+        if (gn.kind == FW_NODE_CUSTOM && !np.custom->vt.process_device) { *why = std::string("custom node '") + np.custom->debug_name + "' has no process_device: it cannot run on the device (there is no CPU fallback)"; return false; }
+        if (needs_mask) {
+            if (n_sum_masks >= (uint32_t)kMaxSumMasks) { *why = "more than 32 mask-dependent nodes in one voice graph"; return false; }
+            gn.mask_slot = (int)n_sum_masks; plan->tables.nodes[i].mask_slot = (uint8_t)(++n_sum_masks);
+        }
+        if (gn.kind == FW_NODE_DUMMY && !endpoint && !sn.out.empty()) { *why = "a DummyAudioNode inside the graph leaves its outputs stale in the reference (dummy.rs:34-41): not reproducible on the device"; return false; }
+        if (gn.kind == FW_NODE_MONO_TO_STEREO && (sn.in.size() != 1 || sn.out.size() != 2)) { *why = "MonoToStereoNode must be 1 -> 2"; return false; }
+        if (gn.kind == FW_NODE_STEREO_TO_MONO && (sn.in.size() != 2 || sn.out.size() != 1)) { *why = "StereoToMonoNode must be 2 -> 1"; return false; }
+        // The program: a copy for graph_in, graph_out and a SumNode (launched by a 1-port one only, sum.rs:58-65), else the node's op. It
+        // runs per channel pair where the body works channel by channel, else once for the node; fuse_generic makes a stereo Volume it
+        // fuses, or that reads the caller's rows, one launch too. With a master bus, the bus stage takes graph_out's channels at once.
+        ChainOp op;
+        if (endpoint || gn.kind == FW_NODE_SUM) {
+            const bool bus_out = bus && i + 1 == n;
+            gn.prog.c_in = gn.prog.c_out = bus_out ? (uint32_t)sn.in.size() : 2u; gn.pairs = !bus_out;
+            if (i == 0) for (uint32_t p = 0; p < sn.out.size(); ++p) gn.src_port.push_back(p);
+        } else if (chain_op(gn.kind, gn.sm0, np.threshold_gain, &op)) {
+            gn.prog.n_ops = 1; gn.prog.ops[0] = op;
+            gn.prog.c_in = gn.kind == FW_NODE_MONO_TO_STEREO ? 1u : 2u; gn.prog.c_out = gn.kind == FW_NODE_STEREO_TO_MONO ? 1u : 2u;
+            gn.pairs = gn.kind == FW_NODE_VOLUME || gn.kind == FW_NODE_HARD_CLIP;
+        }
+        plan->gnodes.push_back(std::move(gn));
+    }
+    plan->rec.n_sum_masks = n_sum_masks;
+    return true;
+}
+
+// Generic lowering, second step (SURVEY f2: "fuse runs of pointwise nodes between fan-out points"):
+//  * a run of mask-independent pointwise nodes (stereo Volume, Pan) that are adjacent in the schedule and feed each other port to
+//    port with no other consumer becomes one chain program, launched where its last node stands; graph_out (copy to the caller's
+//    rows, or the bus stage) can be that last node. Adjacency makes the fused launch read and write its pool buffers at the same
+//    point of the schedule as the unfused nodes did, so the compiler's buffer reuse (compiler.rs:302-412) stays valid; a run whose
+//    last outputs reuse the buffers of its first inputs is not fused (no in-place launches).
+//  * a run head or a Biquad / SVF / Delay node fed entirely by graph_in reads the caller's input rows itself (pointer + pitch),
+//    first-block zeroing after a schedule swap (Q11) included; if every consumer of graph_in does, the pool copy of the inputs is skipped.
+static void fuse_generic(const Schedule& s, Plan* plan) {
+    const size_t n = s.nodes.size();
+    auto& gn = plan->gnodes;
+    std::unordered_map<uint64_t, size_t> index_of;
+    for (size_t i = 0; i < n; ++i) index_of[s.nodes[i].id.pack()] = i;
+    std::vector<std::vector<uint32_t>> n_cons(n);
+    for (size_t i = 0; i < n; ++i) n_cons[i].assign(s.nodes[i].out.size(), 0u);
+    for (size_t i = 0; i < n; ++i) for (const InAssign& a : s.nodes[i].in) {
+        if (a.should_clear) continue;
+        auto it = index_of.find(a.producer.pack());
+        if (it != index_of.end() && a.producer_port < n_cons[it->second].size()) n_cons[it->second][a.producer_port]++;
+    }
+    auto connected = [&](size_t i) { for (const InAssign& a : s.nodes[i].in) if (a.should_clear) return false; return true; };
+    auto stereo_pointwise = [&](size_t i) {
+        return i > 0 && i + 1 < n && (gn[i].kind == FW_NODE_PAN || gn[i].kind == FW_NODE_VOLUME) && s.nodes[i].in.size() == 2 && s.nodes[i].out.size() == 2 &&
+               gn[i].mask_slot < 0 && connected(i);
+    };
+    auto fed_only_by = [&](size_t i, size_t j) {  // node i's inputs are node j's outputs, port to port, and nothing else reads them
+        if (s.nodes[i].in.size() != s.nodes[j].out.size()) return false;
+        for (size_t p = 0; p < s.nodes[i].in.size(); ++p) {
+            const InAssign& a = s.nodes[i].in[p];
+            if (a.should_clear || a.producer != s.nodes[j].id || a.producer_port != p || n_cons[j][p] != 1) return false;
         }
         return true;
     };
-    // Generic lowering, second step (SURVEY f2: "fuse runs of pointwise nodes between fan-out points"):
-    //  * a run of mask-independent pointwise nodes (stereo Volume, Pan) that are adjacent in the schedule and feed each other port to
-    //    port with no other consumer becomes one chain program, launched where its last node stands; graph_out (copy to the caller's
-    //    rows, or the bus stage) can be that last node. Adjacency makes the fused launch read and write its pool buffers at the same
-    //    point of the schedule as the unfused nodes did, so the compiler's buffer reuse (compiler.rs:302-412) stays valid; a run whose
-    //    last outputs reuse the buffers of its first inputs is not fused (no in-place launches).
-    //  * a run head or a Biquad / SVF / Delay node fed entirely by graph_in reads the caller's input rows itself (pointer + pitch),
-    //    first-block zeroing after a schedule swap (Q11) included; if every consumer of graph_in does, the pool copy of the inputs is skipped.
-    auto fuse_generic = [&]() {
-        auto& gn = plan->gnodes;
-        std::unordered_map<uint64_t, size_t> index_of;
-        for (size_t i = 0; i < n; ++i) index_of[s.nodes[i].id.pack()] = i;
-        std::vector<std::vector<uint32_t>> n_cons(n);
-        for (size_t i = 0; i < n; ++i) n_cons[i].assign(s.nodes[i].out.size(), 0u);
-        for (size_t i = 0; i < n; ++i) for (const InAssign& a : s.nodes[i].in) {
-            if (a.should_clear) continue;
-            auto it = index_of.find(a.producer.pack());
-            if (it != index_of.end() && a.producer_port < n_cons[it->second].size()) n_cons[it->second][a.producer_port]++;
-        }
-        auto connected = [&](size_t i) { for (const InAssign& a : s.nodes[i].in) if (a.should_clear) return false; return true; };
-        auto stereo_pointwise = [&](size_t i) {
-            return i > 0 && i + 1 < n && (gn[i].kind == FW_NODE_PAN || gn[i].kind == FW_NODE_VOLUME) && s.nodes[i].in.size() == 2 && s.nodes[i].out.size() == 2 &&
-                   gn[i].mask_slot < 0 && connected(i);
-        };
-        auto fed_only_by = [&](size_t i, size_t j) {  // node i's inputs are node j's outputs, port to port, and nothing else reads them
-            if (s.nodes[i].in.size() != s.nodes[j].out.size()) return false;
-            for (size_t p = 0; p < s.nodes[i].in.size(); ++p) {
-                const InAssign& a = s.nodes[i].in[p];
-                if (a.should_clear || a.producer != s.nodes[j].id || a.producer_port != p || n_cons[j][p] != 1) return false;
-            }
-            return true;
-        };
-        auto op_of = [&](size_t i) { ChainOp op{}; op.sm1 = -1; op.kind = gn[i].kind == FW_NODE_PAN ? OP_PAN : OP_GAIN; op.sm0 = gn[i].sm0; if (gn[i].kind == FW_NODE_PAN) op.sm1 = gn[i].sm1; return op; };
-        // graph_in aliasing: which nodes can read the caller's rows, and is the pool copy still needed
-        std::vector<uint32_t> alias_cons(s.nodes[0].out.size(), 0u);
-        for (size_t i = 1; i + 1 < n; ++i) {
-            const bool temporal = gn[i].kind == FW_NODE_BIQUAD || gn[i].kind == FW_NODE_SVF || gn[i].kind == FW_NODE_DELAY;
-            if (!(stereo_pointwise(i) || (temporal && connected(i) && !s.nodes[i].in.empty()))) continue;
-            bool all = true;
-            for (const InAssign& a : s.nodes[i].in) if (a.producer != s.nodes[0].id || a.producer_port >= alias_cons.size()) all = false;
-            if (!all) continue;
-            for (const InAssign& a : s.nodes[i].in) { gn[i].src_port.push_back(a.producer_port); alias_cons[a.producer_port]++; }
-            plan->reads_caller_rows = true;
-        }
-        plan->gin_copy = false;
-        for (size_t p = 0; p < alias_cons.size(); ++p) if (n_cons[0][p] > alias_cons[p]) plan->gin_copy = true;
-        // runs
-        for (size_t i = 2; i < n; ++i) {
-            const size_t j = i - 1;
-            const bool tail = i + 1 == n && s.nodes[i].in.size() == 2 && !(c->cfg.master_bus && gout.in.size() > 2);
-            if (!(stereo_pointwise(i) || tail) || !stereo_pointwise(j) || !fed_only_by(i, j)) continue;
-            if (gn[j].pre_ops.size() + 2 > (size_t)kMaxChainOps) continue;
-            const std::vector<uint32_t>& head_in = gn[j].run_in.empty() ? gn[j].in_buf : gn[j].run_in;
-            bool in_place = false;
-            if (gn[j].src_port.empty()) for (uint32_t ob : gn[i].out_buf) for (uint32_t ib : head_in) if (ob == ib) in_place = true;
-            if (in_place) continue;
-            gn[i].pre_ops = gn[j].pre_ops; gn[i].pre_ops.push_back(op_of(j));
-            gn[i].run_in = head_in; gn[i].src_port = gn[j].src_port;
-            gn[j].absorbed = true;
-        }
-    };
-    if (!chain_lower()) { if (!generic_lower()) return false; fuse_generic(); }
-    plan->n_sm = n_sm;
+    // graph_in aliasing: which nodes can read the caller's rows, and is the pool copy still needed
+    std::vector<uint32_t> alias_cons(s.nodes[0].out.size(), 0u);
+    for (size_t i = 1; i + 1 < n; ++i) {
+        const bool temporal = gn[i].kind == FW_NODE_BIQUAD || gn[i].kind == FW_NODE_SVF || gn[i].kind == FW_NODE_DELAY;
+        if (!(stereo_pointwise(i) || (temporal && connected(i) && !s.nodes[i].in.empty()))) continue;
+        bool all = true;
+        for (const InAssign& a : s.nodes[i].in) if (a.producer != s.nodes[0].id || a.producer_port >= alias_cons.size()) all = false;
+        if (!all) continue;
+        for (const InAssign& a : s.nodes[i].in) { gn[i].src_port.push_back(a.producer_port); alias_cons[a.producer_port]++; }
+        gn[i].pairs = false;
+        plan->reads_caller_rows = true;
+    }
+    gn[0].absorbed = true;
+    for (size_t p = 0; p < alias_cons.size(); ++p) if (n_cons[0][p] > alias_cons[p]) gn[0].absorbed = false;
+    // runs: node i extends the run that ends at node j = i - 1 by its own op (graph_out adds none)
+    for (size_t i = 2; i < n; ++i) {
+        const size_t j = i - 1;
+        const bool tail = i + 1 == n && s.nodes[i].in.size() == 2;
+        if (!(stereo_pointwise(i) || tail) || !stereo_pointwise(j) || !fed_only_by(i, j)) continue;
+        if (gn[j].prog.n_ops + 1 > (uint32_t)kMaxChainOps) continue;
+        bool in_place = false;
+        if (gn[j].src_port.empty()) for (uint32_t ob : gn[i].out_buf) for (uint32_t ib : gn[j].in_buf) if (ob == ib) in_place = true;
+        if (in_place) continue;
+        ChainProgram pr = gn[j].prog;
+        for (uint32_t k = 0; k < gn[i].prog.n_ops; ++k) pr.ops[pr.n_ops++] = gn[i].prog.ops[k];
+        gn[i].prog = pr; gn[i].pairs = false;
+        gn[i].in_buf = gn[j].in_buf; gn[i].src_port = gn[j].src_port;
+        gn[j].absorbed = true;
+    }
+}
 
-    // ---- device allocations (main thread) ----
-    const uint32_t V = c->cfg.num_voices, F = c->max_block_frames;
+// Device buffers of the plan (main thread): the record buffers, the silence flags and the per-call scratch of one chunk.
+static bool alloc_plan(const fw_ctx* c, Plan* plan, std::string* why) {
+    const uint32_t V = c->cfg.num_voices, F = c->max_block_frames, n_sm = plan->n_sm;
     plan->num_voices = V; plan->block_frames = F; plan->bus = c->cfg.master_bus != 0;
     DevMem& mem = plan->mem;
     plan->d_flags = mem.dev<uint64_t>(V);
@@ -678,7 +703,7 @@ static bool lower(fw_ctx* c, const Schedule& s, Plan* plan, std::string* why) {
     r.gout_mask = mem.dev<uint64_t>(V);
     r.st_modes = mem.dev<uint32_t>(V);
     r.st_vals = mem.dev<float>((size_t)(n_sm ? n_sm : 1) * V);
-    r.n_sum_masks = n_sum_masks;
+    const uint32_t n_sum_masks = r.n_sum_masks;
     r.sum_masks = mem.dev<uint64_t>((size_t)r.kt_max * (n_sum_masks ? n_sum_masks : 1) * V);
     r.st_sum_masks = mem.dev<uint64_t>((size_t)(n_sum_masks ? n_sum_masks : 1) * V);
     r.error = mem.dev<uint32_t>(1);
@@ -701,13 +726,27 @@ static bool lower(fw_ctx* c, const Schedule& s, Plan* plan, std::string* why) {
         r.slot_of = plan->d_slot_of;
     }
     if (!mem.ok()) { *why = "device allocation failed: " + g_dev_err; return false; }
-    plan->tables = tb;
-    {   // delay cursors, reverb history cursors + tensor maps, resampler positions and plugin calls change from call to call
-        bool g = true;
-        for (auto& st : plan->states) if (st->kind == FW_NODE_DELAY || st->kind == FW_NODE_CONV_REVERB || st->kind == FW_NODE_RESAMPLER || st->kind == FW_NODE_CUSTOM) g = false;
-        plan->graphable = g;
-        for (auto& st : plan->states) if (st->kind == FW_NODE_CONV_REVERB) plan->heavy_stage = true;
+    return true;
+}
+
+static bool lower(fw_ctx* c, const Schedule& s, Plan* plan, std::string* why) {
+    std::vector<int> sm_of_node;
+    if (!lower_control(c, s, plan, &sm_of_node, why)) return false;
+    const SchedNode& gin = s.nodes.front();
+    const SchedNode& gout = s.nodes.back();
+    if (gin.out.size() != c->n_in) { *why = "stream input channels must equal the graph_in port count on the device path"; return false; }
+    if (gout.in.size() != c->n_out) { *why = "stream output channels must equal the graph_out port count on the device path"; return false; }
+    plan->c_in = (uint32_t)gin.out.size(); plan->c_out = (uint32_t)gout.in.size();
+    const bool bus = c->cfg.master_bus != 0;
+    if (!lower_chain(s, sm_of_node, bus, plan, why)) {
+        if (!lower_generic(s, sm_of_node, bus, plan, why)) return false;
+        fuse_generic(s, plan);
     }
+    if (!alloc_plan(c, plan, why)) return false;
+    // delay cursors, reverb history cursors + tensor maps, resampler positions and plugin calls change from call to call
+    plan->graphable = true;
+    for (auto& st : plan->states) if (st->kind == FW_NODE_DELAY || st->kind == FW_NODE_CONV_REVERB || st->kind == FW_NODE_RESAMPLER || st->kind == FW_NODE_CUSTOM) plan->graphable = false;
+    for (auto& st : plan->states) if (st->kind == FW_NODE_CONV_REVERB) plan->heavy_stage = true;
     return true;
 }
 
@@ -1387,6 +1426,19 @@ static void proc_poll(fw_processor* p) {  // processor.rs:167-206
 // One chunk of a call: frames [t0, t0 + Tc) of rows that are Tfull frames long in the caller's buffers.
 struct Chunk { uint32_t t0, Tc, Tfull, zero_first; };
 
+// One chain-kernel launch of `prog` over the chunk: channel c of voice v is read at in[c] + v * in_vs and written at out[c] + v * out_vs
+// (floats); an unused second channel repeats channel 0. `caller`: `in` is the caller's rows, whose first block reads as zero after a
+// schedule swap (Q11); otherwise it is the output of the preceding kernel, which the launch waits for.
+static ChainArgs chain_args(const Plan& pl, const Chunk& ck, const ChainProgram& prog, const float* const* in, uint64_t in_vs, float* const* out,
+                            uint64_t out_vs, bool caller) {
+    ChainArgs xa{};
+    xa.in_ch[0] = in[0]; xa.in_ch[1] = in[prog.c_in > 1 ? 1 : 0]; xa.in_vstride = in_vs;
+    xa.out_ch[0] = out[0]; xa.out_ch[1] = out[prog.c_out > 1 ? 1 : 0]; xa.out_vstride = out_vs;
+    xa.num_voices = pl.num_voices; xa.frames = ck.Tc; xa.block_frames = pl.block_frames; xa.zero_first_block = (caller && ck.zero_first) ? 1u : 0u;
+    xa.in_from_prev_kernel = caller ? 0u : 1u; xa.rec = pl.rec; xa.prog = prog;
+    return xa;
+}
+
 // Last stage with a master bus: the chain kernel (BUS variant) reduces 64 voices per CTA into partial buses, the combine
 // kernel finishes the tree, and with several ranks the per-rank buses are exchanged (SURVEY §8e). bus_out = the caller's
 // bus rows (pitch ck.Tfull) at the chunk's first frame.
@@ -1519,32 +1571,6 @@ static int enqueue_generic(fw_processor* p, Plan& pl, const float* d_in, float* 
     auto buf = [&](uint32_t b) { return pl.d_pool + (size_t)b * BS; };
     auto caller_in = [&](size_t c) { return d_in + ck.t0 + c * (size_t)ck.Tfull; };
     if (pl.reads_caller_rows && in_vs > 0xffffffffull) { g_dev_err = "input rows of more than 2^32 / channels frames"; return FW_PROC_BAD_ARGS; }
-    // the inputs of one pointwise launch: up to 2 channels, arbitrary channel pointers; `first`: the caller's rows, not a preceding kernel's output
-    auto chain_args = [&](const ChainProgram& prog, const float* i0, const float* i1, uint64_t ivs, bool first) {
-        ChainArgs xa{};
-        xa.in_ch[0] = i0; xa.in_ch[1] = i1 ? i1 : i0; xa.in_vstride = ivs;
-        xa.num_voices = V; xa.frames = T; xa.block_frames = pl.block_frames; xa.zero_first_block = (first && ck.zero_first) ? 1u : 0u;
-        xa.rec = pl.rec; xa.prog = prog; xa.in_from_prev_kernel = first ? 0u : 1u;
-        return xa;
-    };
-    auto pointwise = [&](ChainArgs xa, float* o0, float* o1, uint64_t ovs) -> bool {
-        xa.out_ch[0] = o0; xa.out_ch[1] = o1 ? o1 : o0; xa.out_vstride = ovs;
-        return FW_LAUNCH(p, 1, 1, launch_chain(xa, false, p->stream));
-    };
-    auto prog1 = [&](int kind, uint32_t ci, uint32_t co, int sm0, int sm1, float f0) {
-        ChainProgram pr{}; pr.c_in = ci; pr.c_out = co; pr.n_ops = kind < 0 ? 0u : 1u;
-        if (kind >= 0) { pr.ops[0].kind = (uint32_t)kind; pr.ops[0].sm0 = sm0; pr.ops[0].sm1 = sm1; pr.ops[0].f0 = f0; }
-        return pr;
-    };
-    // the node's op `kind` (< 0: copy) over nc one-channel blocks, two channels per launch
-    auto per_channel = [&](const Plan::GNode& gn, int kind, const RowBlock* b, size_t nc, bool first) -> bool {
-        for (size_t c = 0; c < nc; c += 2) {
-            const bool two = c + 1 < nc;
-            const ChainArgs xa = chain_args(prog1(kind, two ? 2 : 1, two ? 2 : 1, gn.sm0, gn.sm1, gn.f0), b[c].in, two ? b[c + 1].in : nullptr, b[c].in_pitch, first);
-            if (!pointwise(xa, b[c].out, two ? b[c + 1].out : nullptr, b[c].out_pitch)) return false;
-        }
-        return true;
-    };
     RowBlock rows[64];
     // the node's first n channels as one-channel blocks: inputs from pool buffers or, fed by graph_in, the caller's rows; outputs to pool buffers
     auto node_rows = [&](const Plan::GNode& gn, size_t n) -> const RowBlock* {
@@ -1559,73 +1585,48 @@ static int enqueue_generic(fw_processor* p, Plan& pl, const float* d_in, float* 
         fa.out = buf(gn.out_buf[out_ch]); fa.test = test; fa.num_voices = V; fa.frames = T; fa.block_frames = pl.block_frames; fa.mask_slot = gn.mask_slot; fa.rec = pl.rec;
         return FW_LAUNCH(p, 1, 1, launch_silence_fix(fa, p->stream));
     };
-    // a fused run: the ops of its absorbed nodes + `own` (kind < 0: none), read from the run's first inputs — pool buffers, or the
-    // caller's input channels when the run head is fed by graph_in
-    auto fused_run = [&](const Plan::GNode& gn, int own_kind) {
-        ChainProgram pr{}; pr.c_in = 2; pr.c_out = 2;
-        for (const ChainOp& op : gn.pre_ops) pr.ops[pr.n_ops++] = op;
-        if (own_kind >= 0) { ChainOp& op = pr.ops[pr.n_ops++]; op = ChainOp{}; op.kind = (uint32_t)own_kind; op.sm0 = gn.sm0; op.sm1 = own_kind == OP_PAN ? gn.sm1 : -1; op.f0 = gn.f0; }
-        if (!gn.src_port.empty()) return chain_args(pr, caller_in(gn.src_port[0]), caller_in(gn.src_port[1]), in_vs, true);
-        const std::vector<uint32_t>& ib = gn.run_in.empty() ? gn.in_buf : gn.run_in;
-        return chain_args(pr, buf(ib[0]), buf(ib[1]), T, false);
+    // gn.prog from pool buffers or (src_port) the caller's input rows to pool buffers or, at graph_out, the caller's output rows or the bus stage
+    auto run_prog = [&](const Plan::GNode& gn, bool gout) -> int {
+        const bool caller = !gn.src_port.empty();
+        const size_t ni = caller ? gn.src_port.size() : gn.in_buf.size(), no = gout ? n_out : gn.out_buf.size();
+        const float* in[64] = {}; float* out[64] = {};
+        for (size_t c = 0; c < ni; ++c) in[c] = caller ? caller_in(gn.src_port[c]) : buf(gn.in_buf[c]);
+        const uint64_t ivs = caller ? in_vs : T;
+        if (gout && pl.bus) { ChainArgs xa = chain_args(pl, ck, gn.prog, in, ivs, out, 0, caller); return run_bus_stage(p, pl, xa, n_out, ck, d_out + ck.t0); }
+        for (size_t c = 0; c < no; ++c) out[c] = gout ? d_out + ck.t0 + c * (size_t)ck.Tfull : buf(gn.out_buf[c]);
+        const uint64_t ovs = gout ? out_vs : T;
+        const size_t nc = std::min(ni, no);
+        for (size_t c = 0; c < (gn.pairs ? nc : 1); c += 2) {
+            ChainProgram pr = gn.prog;
+            if (gn.pairs && c + 1 == nc) pr.c_in = pr.c_out = 1;
+            if (!FW_LAUNCH(p, 1, 1, launch_chain(chain_args(pl, ck, pr, in + c, ivs, out + c, ovs, caller), false, p->stream))) return FW_PROC_DEVICE_ERROR;
+        }
+        return FW_PROC_OK;
     };
     const size_t N = pl.gnodes.size();
     for (size_t i = 0; i < N; ++i) {
         Plan::GNode& gn = pl.gnodes[i];
-        if (gn.absorbed) continue;  // runs inside the program of the node that ends its run
+        if (gn.absorbed) continue;  // runs inside the program of the node that ends its run; graph_in: every reader reads the caller's rows
         for (size_t k = 0; k < gn.in_buf.size(); ++k)  // unconnected inputs are cleared every block (schedule.rs:310-313)
             if (gn.in_clear[k]) { if (!FW_CUDA(launch_fill(buf(gn.in_buf[k]), BS, 0.0f, p->stream))) return FW_PROC_DEVICE_ERROR; p->launches++; }
-        if (i == 0) {  // graph_in: stream channels -> pool (prepare_graph_inputs, schedule.rs:213-253)
-            if (!pl.gin_copy) continue;
-            for (size_t c = 0; c < gn.out_buf.size(); ++c) rows[c] = RowBlock{caller_in(c), buf(gn.out_buf[c]), 1, in_vs, T};
-            if (!per_channel(gn, -1, rows, gn.out_buf.size(), true)) return FW_PROC_DEVICE_ERROR;
-            continue;
-        }
-        if (i + 1 == N) {  // graph_out: pool -> stream channels / master bus (read_graph_outputs, schedule.rs:255-287)
-            if (pl.bus) {  // the pointwise run that ends here, if any, rides in the bus stage's program
-                ChainArgs xa = gn.pre_ops.empty() ? chain_args(prog1(-1, n_out, n_out, -1, -1, 0.f), buf(gn.in_buf[0]), buf(gn.in_buf[n_out > 1 ? 1 : 0]), T, false)
-                                                  : fused_run(gn, -1);
-                const int brc = run_bus_stage(p, pl, xa, n_out, ck, d_out + ck.t0);
-                if (brc != FW_PROC_OK) return brc;
-            } else if (!gn.pre_ops.empty()) {
-                float* o0 = d_out + ck.t0;
-                if (!pointwise(fused_run(gn, -1), o0, o0 + ck.Tfull, out_vs)) return FW_PROC_DEVICE_ERROR;
-            } else {
-                for (size_t c = 0; c < gn.in_buf.size(); ++c) rows[c] = RowBlock{buf(gn.in_buf[c]), d_out + ck.t0 + c * (size_t)ck.Tfull, 1, T, out_vs};
-                if (!per_channel(gn, -1, rows, gn.in_buf.size(), false)) return FW_PROC_DEVICE_ERROR;
-            }
-            continue;
-        }
+        // graph_in: stream channels -> pool (prepare_graph_inputs, schedule.rs:213-253); graph_out: pool -> stream channels / master bus
+        // (read_graph_outputs, schedule.rs:255-287)
+        if (i == 0 || i + 1 == N) { const int orc = run_prog(gn, i + 1 == N); if (orc != FW_PROC_OK) return orc; continue; }
         const uint32_t zf = gn.src_port.empty() ? 0u : ck.zero_first;  // Q11 applies to the caller's rows only
-        const size_t n_io = std::min(gn.in_buf.size(), gn.out_buf.size());  // channels of a channel-wise op
         int rc = FW_PROC_OK;
         switch (gn.kind) {
             case FW_NODE_DUMMY: break;  // no outputs (rejected otherwise)
             case FW_NODE_SAMPLER:
                 rc = run_sampler(p, pl, *gn.st, pl.d_srec[gn.sampler_idx], gn.sm0, node_rows(gn, gn.out_buf.size()), (uint32_t)gn.out_buf.size(), T);
                 break;
-            case FW_NODE_VOLUME: case FW_NODE_HARD_CLIP:
-                if (gn.kind == FW_NODE_VOLUME && (!gn.pre_ops.empty() || !gn.src_port.empty())) {  // stereo Volume ending a fused run / reading the caller's rows
-                    if (!pointwise(fused_run(gn, OP_GAIN), buf(gn.out_buf[0]), buf(gn.out_buf[1]), T)) return FW_PROC_DEVICE_ERROR;
-                    break;
-                }
-                if (!per_channel(gn, gn.kind == FW_NODE_VOLUME ? OP_GAIN : OP_CLIP, node_rows(gn, n_io), n_io, false)) return FW_PROC_DEVICE_ERROR;
-                for (size_t c = 0; gn.mask_slot >= 0 && c < gn.out_buf.size(); ++c) if (!silence_fix(gn, c, 1ull << c)) return FW_PROC_DEVICE_ERROR;
-                break;
-            case FW_NODE_PAN:
-                if (!pointwise(fused_run(gn, OP_PAN), buf(gn.out_buf[0]), buf(gn.out_buf[1]), T)) return FW_PROC_DEVICE_ERROR;
-                break;
-            case FW_NODE_MONO_TO_STEREO:
-                if (!pointwise(chain_args(prog1(OP_M2S, 1, 2, -1, -1, 0.f), buf(gn.in_buf[0]), nullptr, T, false), buf(gn.out_buf[0]), buf(gn.out_buf[1]), T)) return FW_PROC_DEVICE_ERROR;
-                if (!silence_fix(gn, 0, 1ull) || !silence_fix(gn, 1, 1ull)) return FW_PROC_DEVICE_ERROR;
-                break;
-            case FW_NODE_STEREO_TO_MONO:
-                if (!pointwise(chain_args(prog1(OP_S2M, 2, 1, -1, -1, 0.f), buf(gn.in_buf[0]), buf(gn.in_buf[1]), T, false), buf(gn.out_buf[0]), nullptr, T)) return FW_PROC_DEVICE_ERROR;
-                if (!silence_fix(gn, 0, 3ull)) return FW_PROC_DEVICE_ERROR;
+            case FW_NODE_VOLUME: case FW_NODE_PAN: case FW_NODE_HARD_CLIP: case FW_NODE_MONO_TO_STEREO: case FW_NODE_STEREO_TO_MONO:
+                rc = run_prog(gn, false);
+                for (size_t c = 0; rc == FW_PROC_OK && gn.mask_slot >= 0 && c < gn.out_buf.size(); ++c)  // test: the inputs output c is made of
+                    if (!silence_fix(gn, c, gn.kind == FW_NODE_STEREO_TO_MONO ? 3ull : gn.kind == FW_NODE_MONO_TO_STEREO ? 1ull : 1ull << c)) return FW_PROC_DEVICE_ERROR;
                 break;
             case FW_NODE_SUM: {
                 const size_t no = gn.out_buf.size(), ports = no ? gn.in_buf.size() / no : 0;
-                if (ports <= 1) { if (!per_channel(gn, -1, node_rows(gn, n_io), n_io, false)) return FW_PROC_DEVICE_ERROR; break; }  // copy (sum.rs:58-65)
+                if (ports <= 1) { rc = run_prog(gn, false); break; }  // copy (sum.rs:58-65)
                 for (size_t c = 0; c < no; ++c) {
                     SumArgs sa{};
                     for (size_t q = 0; q < ports; ++q) { sa.in[q] = buf(gn.in_buf[q * no + c]); sa.mask_bit[q] = (uint8_t)(q * no + c); }
@@ -1778,14 +1779,8 @@ static int enqueue_chunk(fw_processor* p, Plan& pl, const float* d_in, float* d_
             case Plan::STAGE_REVERB: rc = run_reverb(p, *sg.node, &rows, 1, T, zf); break;
             case Plan::STAGE_TEMPORAL: rc = run_temporal(p, sg.node.get(), sg.delay.get(), &rows, 1, T, zf); break;
             case Plan::STAGE_POINTWISE: {
-                ChainArgs xa{};
-                for (uint32_t c = 0; c < 2; ++c) {  // staged chains read / write [V][ch][pitch]
-                    xa.in_ch[c] = src + (size_t)(c < sg.prog.c_in ? c : 0) * src_pitch;
-                    xa.out_ch[c] = dst + (size_t)(c < sg.prog.c_out ? c : 0) * dst_pitch;
-                }
-                xa.in_vstride = (uint64_t)sg.prog.c_in * src_pitch; xa.out_vstride = (uint64_t)sg.prog.c_out * dst_pitch;
-                xa.num_voices = V; xa.frames = T; xa.block_frames = pl.block_frames; xa.zero_first_block = (si == 0 && ck.zero_first) ? 1u : 0u;
-                xa.rec = pl.rec; xa.prog = sg.prog; xa.in_from_prev_kernel = si > 0 ? 1u : 0u;
+                const float* in[2] = {src, src + src_pitch}; float* out[2] = {dst, dst + dst_pitch};  // staged chains read / write [V][ch][pitch]
+                ChainArgs xa = chain_args(pl, ck, sg.prog, in, (uint64_t)sg.prog.c_in * src_pitch, out, (uint64_t)sg.prog.c_out * dst_pitch, si == 0);
                 if (last && pl.bus) rc = run_bus_stage(p, pl, xa, n_out, ck, d_out + ck.t0);
                 else if (!FW_LAUNCH(p, 1, 1, launch_chain(xa, false, p->stream))) rc = FW_PROC_DEVICE_ERROR;
                 break;
