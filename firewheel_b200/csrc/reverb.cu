@@ -90,11 +90,12 @@ __global__ void reverb_prepare(const float* __restrict__ in, __nv_bfloat16* __re
     const uint32_t c = row / V, v = row % V;
     __nv_bfloat16* dst = xh + ((size_t)chan_base * V + row) * pitch + cursor;
     const float* x = in + ((size_t)v * C + c) * in_pitch;
-    const bool vec = (T % 8u) == 0 && (in_pitch % 4u) == 0 && (cursor % 8u) == 0 && (pitch % 8u) == 0 && (reinterpret_cast<uintptr_t>(in) % 16u) == 0;
+    const bool vec = (T % 8u) == 0 && (zero_first % 8u) == 0 && (in_pitch % 4u) == 0 && (cursor % 8u) == 0 && (pitch % 8u) == 0 &&
+                     (reinterpret_cast<uintptr_t>(in) % 16u) == 0;
     if (vec) {
         for (uint32_t i = (blockIdx.y * blockDim.x + threadIdx.x) * 8u; i < T; i += gridDim.y * blockDim.x * 8u) {
             float4 a = __ldcs(reinterpret_cast<const float4*>(x + i)), b = __ldcs(reinterpret_cast<const float4*>(x + i + 4));
-            if (i < zero_first) { a = make_float4(0.f, 0.f, 0.f, 0.f); b = a; }  // zero_first is a multiple of the block size here
+            if (i < zero_first) { a = make_float4(0.f, 0.f, 0.f, 0.f); b = a; }
             __nv_bfloat162 p0 = __floats2bfloat162_rn(a.x, a.y), p1 = __floats2bfloat162_rn(a.z, a.w), p2 = __floats2bfloat162_rn(b.x, b.y), p3 = __floats2bfloat162_rn(b.z, b.w);
             uint4 o;
             o.x = *reinterpret_cast<uint32_t*>(&p0); o.y = *reinterpret_cast<uint32_t*>(&p1); o.z = *reinterpret_cast<uint32_t*>(&p2); o.w = *reinterpret_cast<uint32_t*>(&p3);

@@ -1538,26 +1538,29 @@ static int run_temporal(fw_processor* p, const NodeDeviceState* filter, NodeDevi
 }
 
 // ConvReverb: one history + GEMM launch per block; history rows of channel c are c * V .. c * V + V - 1. The history cursor
-// advances once per chunk, the GEMM's fix-up epoch once per launch.
+// advances once per piece, the GEMM's fix-up epoch once per launch. A chunk longer than the history buffers hold
+// (kReverbMaxFrames) is processed as consecutive pieces of at most that many frames.
 static int run_reverb(fw_processor* p, NodeDeviceState& rs, const RowBlock* b, uint32_t nb, uint32_t T, uint32_t zero_first) {
-    if (T > NodeDeviceState::kReverbMaxFrames) { g_dev_err = "conv reverb: more than 65536 frames in one chunk"; return FW_PROC_BAD_ARGS; }
     const uint32_t V = p->num_voices, H = reverb_hist(rs.params->ir_len);
-    if (rs.xh_cursor + T > rs.xh_pitch || (rs.xh_cursor & 7u)) {  // buffer full (or cursor off the 16-byte TMA grid after an odd-length call):
-        // carry the H most recent samples to the front of the other buffer
-        if (!FW_CUDA(cudaMemcpy2DAsync(rs.d_xh[rs.xh_cur ^ 1u], (size_t)rs.xh_pitch * 2, static_cast<const uint16_t*>(rs.d_xh[rs.xh_cur]) + (rs.xh_cursor - H),
-                                       (size_t)rs.xh_pitch * 2, (size_t)H * 2, (size_t)V * channels_of(b, nb), cudaMemcpyDeviceToDevice, p->stream))) return FW_PROC_DEVICE_ERROR;
-        rs.xh_cur ^= 1u; rs.xh_cursor = H;
+    for (uint32_t t0 = 0; t0 < T; t0 += NodeDeviceState::kReverbMaxFrames) {
+        const uint32_t Tp = std::min(T - t0, NodeDeviceState::kReverbMaxFrames), zf = zero_first > t0 ? std::min(zero_first - t0, Tp) : 0u;
+        if (rs.xh_cursor + Tp > rs.xh_pitch || (rs.xh_cursor & 7u)) {  // buffer full (or cursor off the 16-byte TMA grid after an odd-length piece):
+            // carry the H most recent samples to the front of the other buffer
+            if (!FW_CUDA(cudaMemcpy2DAsync(rs.d_xh[rs.xh_cur ^ 1u], (size_t)rs.xh_pitch * 2, static_cast<const uint16_t*>(rs.d_xh[rs.xh_cur]) + (rs.xh_cursor - H),
+                                           (size_t)rs.xh_pitch * 2, (size_t)H * 2, (size_t)V * channels_of(b, nb), cudaMemcpyDeviceToDevice, p->stream))) return FW_PROC_DEVICE_ERROR;
+            rs.xh_cur ^= 1u; rs.xh_cursor = H;
+        }
+        for (uint32_t i = 0, c = 0; i < nb; c += b[i].C, ++i) {
+            ReverbCall rc{};
+            rc.in = b[i].in + t0; rc.out = b[i].out + t0; rc.in_pitch = (uint32_t)b[i].in_pitch; rc.out_pitch = (uint32_t)b[i].out_pitch; rc.xh = rs.d_xh[rs.xh_cur]; rc.bt = rs.d_bt;
+            rc.V = V; rc.C = b[i].C; rc.T = Tp; rc.L = rs.params->ir_len; rc.ir_ch = rs.params->ir_channels; rc.cursor = rs.xh_cursor; rc.pitch = rs.xh_pitch;
+            rc.zero_first = zf; rc.chan_base = c;
+            rc.ws = rs.d_rv_ws; rc.flags = rs.d_rv_flags; rc.epoch = ++rs.rv_epoch;
+            std::string rerr;
+            if (!FW_LAUNCH(p, 3, 2, launch_reverb(rc, p->stream, &rerr))) { if (!rerr.empty()) g_dev_err = rerr; return FW_PROC_DEVICE_ERROR; }
+        }
+        rs.xh_cursor += Tp;
     }
-    for (uint32_t i = 0, c = 0; i < nb; c += b[i].C, ++i) {
-        ReverbCall rc{};
-        rc.in = b[i].in; rc.out = b[i].out; rc.in_pitch = (uint32_t)b[i].in_pitch; rc.out_pitch = (uint32_t)b[i].out_pitch; rc.xh = rs.d_xh[rs.xh_cur]; rc.bt = rs.d_bt;
-        rc.V = V; rc.C = b[i].C; rc.T = T; rc.L = rs.params->ir_len; rc.ir_ch = rs.params->ir_channels; rc.cursor = rs.xh_cursor; rc.pitch = rs.xh_pitch;
-        rc.zero_first = zero_first; rc.chan_base = c;
-        rc.ws = rs.d_rv_ws; rc.flags = rs.d_rv_flags; rc.epoch = ++rs.rv_epoch;
-        std::string rerr;
-        if (!FW_LAUNCH(p, 3, 2, launch_reverb(rc, p->stream, &rerr))) { if (!rerr.empty()) g_dev_err = rerr; return FW_PROC_DEVICE_ERROR; }
-    }
-    rs.xh_cursor += T;
     return FW_PROC_OK;
 }
 
