@@ -269,22 +269,25 @@ struct Plan {
     std::vector<std::shared_ptr<NodeDeviceState>> states;   // keeps every referenced node state alive
     std::vector<Id> nodes_to_remove;
     CtlTables tables{}; uint64_t* d_flags = nullptr;
-    // data plane: stages run in order; pointwise stages are fused chain programs, the others own state
-    enum StageKind { STAGE_POINTWISE, STAGE_TEMPORAL, STAGE_REVERB, STAGE_SAMPLER };  // STAGE_SAMPLER: a SamplerNode heading the chain
-    // node: the biquad or SVF of a temporal stage (none: a lone delay), the reverb, the sampler; delay: a temporal stage's delay line
-    struct Stage { StageKind kind = STAGE_POINTWISE; ChainProgram prog{}; uint32_t c_in = 0, c_out = 0;
-                   std::shared_ptr<NodeDeviceState> node, delay; int sampler_sm = -1; };
-    std::vector<Stage> stages;
-    // generic lowering (arbitrary DAG of built-in nodes): one launch group per scheduled node over pool buffers [buffer][V][T]
-    struct GNode { uint32_t kind = 0; std::vector<uint32_t> in_buf, out_buf; std::vector<uint8_t> in_clear; int sm0 = -1, mask_slot = -1, custom_idx = -1, sampler_idx = -1;
-                   std::shared_ptr<NodeDeviceState> st;
-                   // graph_in, graph_out and pointwise nodes launch `prog`, once or (`pairs`) per channel pair, an odd last channel narrowed
-                   // to 1 -> 1. Fusion and graph_in aliasing (see fuse_generic): a run of stereo Volume / Pan nodes, optionally ending in
-                   // graph_out, is ONE program launched at its last node, which then reads the run's first inputs (in_buf); the others are
-                   // `absorbed`, and so is graph_in when no node reads its pool copy. `src_port` non-empty: the node (or its run) reads the
-                   // caller's input channels src_port[k] instead of pool buffers.
-                   ChainProgram prog{}; bool pairs = false, absorbed = false; std::vector<uint32_t> src_port; };
-    bool generic = false; std::vector<GNode> gnodes; uint32_t num_buffers = 0;
+    // Data plane: the steps run in order, each one launch group. An operand is C contiguous channels of one space: the caller's input or
+    // output rows from channel `index` (row pitch Tfull, or n_in / n_out * Tfull for C == 1), pool buffer `index` of the generic lowering
+    // ([buffer][V][chunk], C == 1), or inter-stage scratch d_tmp[index] of the fused chain ([V][C][chunk]).
+    enum Space : uint8_t { CALLER_IN, CALLER_OUT, POOL, SCRATCH };
+    struct Operand { Space space; uint32_t index, C; };
+    struct Step {
+        enum Kind : uint8_t { PROG, SAMPLER, TEMPORAL, REVERB, SUM, RESAMPLER, CUSTOM } kind = PROG;
+        // node: the sampler, the biquad or SVF of a temporal step (none: a lone delay), the reverb, resampler or custom node; delay: a
+        // temporal step's delay line
+        std::shared_ptr<NodeDeviceState> node, delay;
+        // PROG launches `prog` once or (`pairs`) per channel pair, an odd last channel narrowed to 1 -> 1. On a master-bus plan the last
+        // step is a PROG whose voices run_bus_stage sums into the bus; the generic lowering gives it no output operands.
+        ChainProgram prog{}; bool pairs = false;
+        int sm0 = -1, sampler_idx = -1, mask_slot = -1, custom_idx = -1;
+        std::vector<uint32_t> clear;          // pool buffers cleared before the step: unconnected inputs (schedule.rs:310-313)
+        std::vector<Operand> in, out;
+    };
+    std::vector<Step> steps;
+    uint32_t num_buffers = 0;  // generic lowering: pool buffers
     bool reads_caller_rows = false;  // some node reads the caller's input rows directly (row pitch n_in * frames must fit 32 bits)
     std::vector<std::shared_ptr<NodeDeviceState>> samplers;  // index = CtlTables::smp index
     std::vector<std::shared_ptr<NodeDeviceState>> resamplers;  // index = CtlTables::rs index
@@ -301,7 +304,7 @@ struct Plan {
     float* d_pool = nullptr;                   // generic lowering: [buffer][V][chunk]
     uint16_t* d_slot_of = nullptr;             // sampler graphs: record slot per (block, voice)
     std::vector<SmpRec*> d_srec;               // per SamplerNode: [block][voice]
-    std::vector<uint64_t*> d_custom_masks;     // per custom node (index = GNode::custom_idx): dense [block][voice] input masks
+    std::vector<uint64_t*> d_custom_masks;     // per custom node (index = Step::custom_idx): dense [block][voice] input masks
     DevMem mem;  // d_flags, the records, d_bus_mask and the scratch; declared last so that it frees them before the node states go
 };
 
@@ -487,20 +490,29 @@ static bool lower_control(fw_ctx* c, const Schedule& s, Plan* plan, std::vector<
     return true;
 }
 
-// Data plane, first choice: a linear chain graph_in -> n1 -> ... -> nk -> graph_out, port i to port i, fused into stages. False, with
-// the reason, for any other schedule.
+// Data plane, first choice: a linear chain graph_in -> n1 -> ... -> nk -> graph_out, port i to port i, fused into stages. Stage 0
+// reads the caller's rows, stage si writes scratch si & 1 and the last stage the caller's output rows. False, with the reason, for
+// any other schedule.
 static bool lower_chain(const Schedule& s, const std::vector<int>& sm_of_node, bool bus, Plan* plan, std::string* why) {
     const size_t n = s.nodes.size();
     const SchedNode& gin = s.nodes.front();
     const SchedNode& gout = s.nodes.back();
+    std::vector<Plan::Step>& steps = plan->steps;
     uint32_t width = (uint32_t)gin.out.size();
+    // a stage of `width` channels in and out (the space and index of its operands are set at the end)
+    auto stage = [&](Plan::Step::Kind kind, const std::shared_ptr<NodeDeviceState>& node) {
+        Plan::Step sp; sp.kind = kind; sp.node = node;
+        sp.in = {Plan::Operand{Plan::SCRATCH, 0, width}}; sp.out = sp.in;
+        steps.push_back(std::move(sp));
+    };
     Id prev = gin.id;
     size_t first = 1;
     if (width == 0 && n >= 3 && plan->tables.nodes[1].kind == FW_NODE_SAMPLER && s.nodes[1].in.empty() && s.nodes[1].out.size() >= 1 && s.nodes[1].out.size() <= 2) {
         // no stream inputs: a SamplerNode heads the chain (BASELINE config 5: sampler -> gain -> pan -> ... -> bus)
-        Plan::Stage hs; hs.kind = Plan::STAGE_SAMPLER; hs.c_in = 0; hs.c_out = (uint32_t)s.nodes[1].out.size(); hs.node = plan->states[1]; hs.sampler_sm = sm_of_node[1];
-        plan->stages.push_back(hs);
-        width = hs.c_out; prev = s.nodes[1].id; first = 2;
+        width = (uint32_t)s.nodes[1].out.size();
+        stage(Plan::Step::SAMPLER, plan->states[1]);
+        steps.back().in.clear(); steps.back().sm0 = sm_of_node[1]; steps.back().sampler_idx = plan->tables.nodes[1].sm1;
+        prev = s.nodes[1].id; first = 2;
     }
     if (width < 1 || width > 2) { *why = "the fused chain supports 1 or 2 channels"; return false; }
     auto fed_by_prev = [&](const SchedNode& sn, uint32_t w) {
@@ -508,11 +520,10 @@ static bool lower_chain(const Schedule& s, const std::vector<int>& sm_of_node, b
         for (uint32_t p = 0; p < w; ++p) if (sn.in[p].should_clear || sn.in[p].producer != prev || sn.in[p].producer_port != p) return false;
         return true;
     };
-    Plan::Stage cur; cur.prog.c_in = width; cur.c_in = width;
-    bool cur_open = true;  // a pointwise stage is being accumulated
+    ChainProgram cur{}; cur.c_in = width;  // the pointwise stage being accumulated
     auto close_pointwise = [&](bool force) {
-        if (cur_open && (cur.prog.n_ops > 0 || force)) { cur.prog.c_out = width; cur.c_out = width; plan->stages.push_back(cur); }
-        cur = Plan::Stage{}; cur.prog.c_in = width; cur.c_in = width; cur_open = true;
+        if (cur.n_ops > 0 || force) { cur.c_out = width; stage(Plan::Step::PROG, nullptr); steps.back().prog = cur; steps.back().in[0].C = cur.c_in; }
+        cur = ChainProgram{}; cur.c_in = width;
     };
     for (size_t i = first; i + 1 < n; ++i) {
         const SchedNode& sn = s.nodes[i];
@@ -520,95 +531,94 @@ static bool lower_chain(const Schedule& s, const std::vector<int>& sm_of_node, b
         if (!fed_by_prev(sn, width)) { *why = "voice graph is not a linear port-to-port chain"; return false; }
         if (sn.out.size() < 1 || sn.out.size() > 2) { *why = "the fused chain supports 1 or 2 channels"; return false; }
         const uint32_t kind = np.kind;
-        if (kind == FW_NODE_CONV_REVERB) {
-            close_pointwise(false);
-            Plan::Stage ts; ts.kind = Plan::STAGE_REVERB; ts.c_in = ts.c_out = width; ts.node = plan->states[i];
-            plan->stages.push_back(ts);
-            prev = sn.id;
-            continue;
-        }
-        if (kind == FW_NODE_SVF) {
-            close_pointwise(false);
-            Plan::Stage ts; ts.kind = Plan::STAGE_TEMPORAL; ts.c_in = ts.c_out = width; ts.node = plan->states[i];
-            plan->stages.push_back(ts);
-            prev = sn.id;
-            continue;
-        }
-        if (kind == FW_NODE_BIQUAD || kind == FW_NODE_DELAY) {
+        if (kind == FW_NODE_CONV_REVERB || kind == FW_NODE_SVF || kind == FW_NODE_BIQUAD || kind == FW_NODE_DELAY) {
             const std::shared_ptr<NodeDeviceState>& st = plan->states[i];
-            // a delay directly after a biquad joins its pass; anything else opens a new temporal stage
-            if (kind == FW_NODE_DELAY && !plan->stages.empty() && plan->stages.back().kind == Plan::STAGE_TEMPORAL && !plan->stages.back().delay &&
-                plan->stages.back().node && plan->stages.back().node->kind == FW_NODE_BIQUAD && cur.prog.n_ops == 0) {
-                plan->stages.back().delay = st;
+            // a delay directly after a biquad joins its pass; anything else opens a new stage
+            if (kind == FW_NODE_DELAY && !steps.empty() && steps.back().kind == Plan::Step::TEMPORAL && !steps.back().delay &&
+                steps.back().node && steps.back().node->kind == FW_NODE_BIQUAD && cur.n_ops == 0) {
+                steps.back().delay = st;
             } else {
                 close_pointwise(false);
-                Plan::Stage ts; ts.kind = Plan::STAGE_TEMPORAL; ts.c_in = ts.c_out = width;
-                if (kind == FW_NODE_BIQUAD) ts.node = st; else ts.delay = st;
-                plan->stages.push_back(ts);
+                stage(kind == FW_NODE_CONV_REVERB ? Plan::Step::REVERB : Plan::Step::TEMPORAL, kind == FW_NODE_DELAY ? nullptr : st);
+                if (kind == FW_NODE_DELAY) steps.back().delay = st;
             }
             prev = sn.id;
             continue;
         }
-        if (cur.prog.n_ops >= (uint32_t)kMaxChainOps) { *why = "more than 16 pointwise nodes in a row"; return false; }
+        if (cur.n_ops >= (uint32_t)kMaxChainOps) { *why = "more than 16 pointwise nodes in a row"; return false; }
         if (kind == FW_NODE_SUM) {
             if (sn.in.size() == sn.out.size()) { prev = sn.id; continue; }  // 1-port sum == copy (sum.rs:58-65): no data op
             *why = "SumNode with more than one port inside a voice chain"; return false;
         }
         ChainOp op;
         if (!chain_op(kind, sm_of_node[i], np.threshold_gain, &op)) { *why = std::string("node kind '") + node_debug_name(kind) + "' has no device lowering yet"; return false; }
-        cur.prog.ops[cur.prog.n_ops++] = op;
+        cur.ops[cur.n_ops++] = op;
         width = (uint32_t)sn.out.size();
         prev = sn.id;
     }
     if (!fed_by_prev(gout, width)) { *why = "graph_out is not fed port-to-port by the end of the chain"; return false; }
     // the last stage must be pointwise when the master bus follows it, and a plan is never empty
-    close_pointwise(plan->stages.empty() || (bus && cur.prog.n_ops == 0 && plan->stages.back().kind != Plan::STAGE_POINTWISE));
+    close_pointwise(steps.empty() || (bus && cur.n_ops == 0 && steps.back().kind != Plan::Step::PROG));
+    for (uint32_t si = 0; si < steps.size(); ++si) {
+        const bool last = si + 1 == steps.size();
+        for (Plan::Operand& o : steps[si].in) o = si == 0 ? Plan::Operand{Plan::CALLER_IN, 0, o.C} : Plan::Operand{Plan::SCRATCH, (si - 1) & 1, o.C};
+        for (Plan::Operand& o : steps[si].out) o = last ? Plan::Operand{Plan::CALLER_OUT, 0, o.C} : Plan::Operand{Plan::SCRATCH, si & 1, o.C};
+    }
     plan->c_out = width;
     return true;
 }
 
-// Data plane, general case: the reference's own buffer assignment on device, one launch group per scheduled node. graph_in, graph_out
-// and the pointwise nodes get the chain program they launch.
+// Data plane, general case: the reference's own buffer assignment on device, one step per scheduled node over pool buffers. graph_in
+// copies the caller's rows to the pool, graph_out the pool to the caller's rows or the bus (prepare_graph_inputs / read_graph_outputs,
+// schedule.rs:213-287).
 static bool lower_generic(const Schedule& s, const std::vector<int>& sm_of_node, bool bus, Plan* plan, std::string* why) {
     const size_t n = s.nodes.size();
-    plan->stages.clear(); plan->generic = true; plan->num_buffers = s.num_buffers;
+    plan->steps.clear(); plan->num_buffers = s.num_buffers;
     if (bus && s.nodes.back().in.size() > 2) { *why = "master bus over more than 2 graph_out channels"; return false; }
     uint32_t n_sum_masks = 0;  // nodes whose data-plane body needs the per-block input silence mask
     for (size_t i = 0; i < n; ++i) {
         const SchedNode& sn = s.nodes[i];
         const NodeParams& np = *plan->states[i]->params;
-        Plan::GNode gn; gn.kind = np.kind; gn.st = plan->states[i];
-        for (const InAssign& a : sn.in) { gn.in_buf.push_back(a.buffer); gn.in_clear.push_back(a.should_clear); }
-        for (const OutAssign& a : sn.out) gn.out_buf.push_back(a.buffer);
-        gn.sm0 = sm_of_node[i];
-        if (gn.kind == FW_NODE_SAMPLER) gn.sampler_idx = plan->tables.nodes[i].sm1;
+        const uint32_t kind = np.kind;
         const bool endpoint = i == 0 || i + 1 == n;
+        Plan::Step sp; sp.node = plan->states[i]; sp.sm0 = sm_of_node[i];
+        for (const InAssign& a : sn.in) { sp.in.push_back(Plan::Operand{Plan::POOL, a.buffer, 1}); if (a.should_clear) sp.clear.push_back(a.buffer); }
+        for (const OutAssign& a : sn.out) sp.out.push_back(Plan::Operand{Plan::POOL, a.buffer, 1});
+        if (i == 0) for (uint32_t p = 0; p < sn.out.size(); ++p) sp.in.push_back(Plan::Operand{Plan::CALLER_IN, p, 1});
+        if (i + 1 == n && !bus) for (uint32_t p = 0; p < sn.in.size(); ++p) sp.out.push_back(Plan::Operand{Plan::CALLER_OUT, p, 1});
         // bodies that branch on the input silence mask (see silence_fix_kernel / sum_kernel)
-        const bool needs_mask = !endpoint && ((gn.kind == FW_NODE_CUSTOM) || (!sn.out.empty() &&
-            ((gn.kind == FW_NODE_SUM && sn.in.size() != sn.out.size()) || gn.kind == FW_NODE_HARD_CLIP || (gn.kind == FW_NODE_VOLUME && sn.in.size() != 2) ||
-             gn.kind == FW_NODE_MONO_TO_STEREO || gn.kind == FW_NODE_STEREO_TO_MONO)));
-        if (gn.kind == FW_NODE_CUSTOM && !np.custom->vt.process_device) { *why = std::string("custom node '") + np.custom->debug_name + "' has no process_device: it cannot run on the device (there is no CPU fallback)"; return false; }
+        const bool needs_mask = !endpoint && ((kind == FW_NODE_CUSTOM) || (!sn.out.empty() &&
+            ((kind == FW_NODE_SUM && sn.in.size() != sn.out.size()) || kind == FW_NODE_HARD_CLIP || (kind == FW_NODE_VOLUME && sn.in.size() != 2) ||
+             kind == FW_NODE_MONO_TO_STEREO || kind == FW_NODE_STEREO_TO_MONO)));
+        if (kind == FW_NODE_CUSTOM && !np.custom->vt.process_device) { *why = std::string("custom node '") + np.custom->debug_name + "' has no process_device: it cannot run on the device (there is no CPU fallback)"; return false; }
         if (needs_mask) {
             if (n_sum_masks >= (uint32_t)kMaxSumMasks) { *why = "more than 32 mask-dependent nodes in one voice graph"; return false; }
-            gn.mask_slot = (int)n_sum_masks; plan->tables.nodes[i].mask_slot = (uint8_t)(++n_sum_masks);
+            sp.mask_slot = (int)n_sum_masks; plan->tables.nodes[i].mask_slot = (uint8_t)(++n_sum_masks);
         }
-        if (gn.kind == FW_NODE_DUMMY && !endpoint && !sn.out.empty()) { *why = "a DummyAudioNode inside the graph leaves its outputs stale in the reference (dummy.rs:34-41): not reproducible on the device"; return false; }
-        if (gn.kind == FW_NODE_MONO_TO_STEREO && (sn.in.size() != 1 || sn.out.size() != 2)) { *why = "MonoToStereoNode must be 1 -> 2"; return false; }
-        if (gn.kind == FW_NODE_STEREO_TO_MONO && (sn.in.size() != 2 || sn.out.size() != 1)) { *why = "StereoToMonoNode must be 2 -> 1"; return false; }
-        // The program: a copy for graph_in, graph_out and a SumNode (launched by a 1-port one only, sum.rs:58-65), else the node's op. It
-        // runs per channel pair where the body works channel by channel, else once for the node; fuse_generic makes a stereo Volume it
-        // fuses, or that reads the caller's rows, one launch too. With a master bus, the bus stage takes graph_out's channels at once.
+        if (kind == FW_NODE_DUMMY && !endpoint && !sn.out.empty()) { *why = "a DummyAudioNode inside the graph leaves its outputs stale in the reference (dummy.rs:34-41): not reproducible on the device"; return false; }
+        if (kind == FW_NODE_MONO_TO_STEREO && (sn.in.size() != 1 || sn.out.size() != 2)) { *why = "MonoToStereoNode must be 1 -> 2"; return false; }
+        if (kind == FW_NODE_STEREO_TO_MONO && (sn.in.size() != 2 || sn.out.size() != 1)) { *why = "StereoToMonoNode must be 2 -> 1"; return false; }
+        // The program: a copy for graph_in, graph_out (both Dummy nodes), a 1-port SumNode (sum.rs:58-65) and a Dummy node inside the
+        // graph, which has no outputs and so launches nothing; else the node's op. It runs per channel pair where the body works channel
+        // by channel, else once for the node; fuse_generic makes a stereo Volume it fuses, or that reads the caller's rows, one launch
+        // too. With a master bus, the bus stage takes graph_out's channels at once.
         ChainOp op;
-        if (endpoint || gn.kind == FW_NODE_SUM) {
+        if (kind == FW_NODE_DUMMY || (kind == FW_NODE_SUM && sn.in.size() == sn.out.size())) {
             const bool bus_out = bus && i + 1 == n;
-            gn.prog.c_in = gn.prog.c_out = bus_out ? (uint32_t)sn.in.size() : 2u; gn.pairs = !bus_out;
-            if (i == 0) for (uint32_t p = 0; p < sn.out.size(); ++p) gn.src_port.push_back(p);
-        } else if (chain_op(gn.kind, gn.sm0, np.threshold_gain, &op)) {
-            gn.prog.n_ops = 1; gn.prog.ops[0] = op;
-            gn.prog.c_in = gn.kind == FW_NODE_MONO_TO_STEREO ? 1u : 2u; gn.prog.c_out = gn.kind == FW_NODE_STEREO_TO_MONO ? 1u : 2u;
-            gn.pairs = gn.kind == FW_NODE_VOLUME || gn.kind == FW_NODE_HARD_CLIP;
+            sp.prog.c_in = sp.prog.c_out = bus_out ? (uint32_t)sn.in.size() : 2u; sp.pairs = !bus_out;
+        } else if (chain_op(kind, sp.sm0, np.threshold_gain, &op)) {
+            sp.prog.n_ops = 1; sp.prog.ops[0] = op;
+            sp.prog.c_in = kind == FW_NODE_MONO_TO_STEREO ? 1u : 2u; sp.prog.c_out = kind == FW_NODE_STEREO_TO_MONO ? 1u : 2u;
+            sp.pairs = kind == FW_NODE_VOLUME || kind == FW_NODE_HARD_CLIP;
+        } else if (kind == FW_NODE_BIQUAD || kind == FW_NODE_SVF || kind == FW_NODE_DELAY) {
+            sp.kind = Plan::Step::TEMPORAL;
+            if (kind == FW_NODE_DELAY) std::swap(sp.node, sp.delay);
+        } else {
+            sp.kind = kind == FW_NODE_SUM ? Plan::Step::SUM : kind == FW_NODE_SAMPLER ? Plan::Step::SAMPLER : kind == FW_NODE_CONV_REVERB ? Plan::Step::REVERB :
+                      kind == FW_NODE_RESAMPLER ? Plan::Step::RESAMPLER : Plan::Step::CUSTOM;
+            if (kind == FW_NODE_SAMPLER) sp.sampler_idx = plan->tables.nodes[i].sm1;
         }
-        plan->gnodes.push_back(std::move(gn));
+        plan->steps.push_back(std::move(sp));
     }
     plan->rec.n_sum_masks = n_sum_masks;
     return true;
@@ -624,7 +634,8 @@ static bool lower_generic(const Schedule& s, const std::vector<int>& sm_of_node,
 //    first-block zeroing after a schedule swap (Q11) included; if every consumer of graph_in does, the pool copy of the inputs is skipped.
 static void fuse_generic(const Schedule& s, Plan* plan) {
     const size_t n = s.nodes.size();
-    auto& gn = plan->gnodes;
+    std::vector<Plan::Step>& st = plan->steps;  // one per scheduled node until the end
+    auto kind = [&](size_t i) { return plan->states[i]->kind; };
     std::unordered_map<uint64_t, size_t> index_of;
     for (size_t i = 0; i < n; ++i) index_of[s.nodes[i].id.pack()] = i;
     std::vector<std::vector<uint32_t>> n_cons(n);
@@ -636,8 +647,8 @@ static void fuse_generic(const Schedule& s, Plan* plan) {
     }
     auto connected = [&](size_t i) { for (const InAssign& a : s.nodes[i].in) if (a.should_clear) return false; return true; };
     auto stereo_pointwise = [&](size_t i) {
-        return i > 0 && i + 1 < n && (gn[i].kind == FW_NODE_PAN || gn[i].kind == FW_NODE_VOLUME) && s.nodes[i].in.size() == 2 && s.nodes[i].out.size() == 2 &&
-               gn[i].mask_slot < 0 && connected(i);
+        return i > 0 && i + 1 < n && (kind(i) == FW_NODE_PAN || kind(i) == FW_NODE_VOLUME) && s.nodes[i].in.size() == 2 && s.nodes[i].out.size() == 2 &&
+               st[i].mask_slot < 0 && connected(i);
     };
     auto fed_only_by = [&](size_t i, size_t j) {  // node i's inputs are node j's outputs, port to port, and nothing else reads them
         if (s.nodes[i].in.size() != s.nodes[j].out.size()) return false;
@@ -647,39 +658,47 @@ static void fuse_generic(const Schedule& s, Plan* plan) {
         }
         return true;
     };
+    std::vector<bool> folded(n, false);  // runs inside the step that ends its run; graph_in: every reader reads the caller's rows
     // graph_in aliasing: which nodes can read the caller's rows, and is the pool copy still needed
     std::vector<uint32_t> alias_cons(s.nodes[0].out.size(), 0u);
     for (size_t i = 1; i + 1 < n; ++i) {
-        const bool temporal = gn[i].kind == FW_NODE_BIQUAD || gn[i].kind == FW_NODE_SVF || gn[i].kind == FW_NODE_DELAY;
+        const bool temporal = kind(i) == FW_NODE_BIQUAD || kind(i) == FW_NODE_SVF || kind(i) == FW_NODE_DELAY;
         if (!(stereo_pointwise(i) || (temporal && connected(i) && !s.nodes[i].in.empty()))) continue;
         bool all = true;
         for (const InAssign& a : s.nodes[i].in) if (a.producer != s.nodes[0].id || a.producer_port >= alias_cons.size()) all = false;
         if (!all) continue;
-        for (const InAssign& a : s.nodes[i].in) { gn[i].src_port.push_back(a.producer_port); alias_cons[a.producer_port]++; }
-        gn[i].pairs = false;
+        for (size_t k = 0; k < s.nodes[i].in.size(); ++k) {
+            const uint32_t port = s.nodes[i].in[k].producer_port;
+            st[i].in[k] = Plan::Operand{Plan::CALLER_IN, port, 1};
+            alias_cons[port]++;
+        }
+        st[i].pairs = false;
         plan->reads_caller_rows = true;
     }
-    gn[0].absorbed = true;
-    for (size_t p = 0; p < alias_cons.size(); ++p) if (n_cons[0][p] > alias_cons[p]) gn[0].absorbed = false;
+    folded[0] = true;
+    for (size_t p = 0; p < alias_cons.size(); ++p) if (n_cons[0][p] > alias_cons[p]) folded[0] = false;
     // runs: node i extends the run that ends at node j = i - 1 by its own op (graph_out adds none)
     for (size_t i = 2; i < n; ++i) {
         const size_t j = i - 1;
         const bool tail = i + 1 == n && s.nodes[i].in.size() == 2;
         if (!(stereo_pointwise(i) || tail) || !stereo_pointwise(j) || !fed_only_by(i, j)) continue;
-        if (gn[j].prog.n_ops + 1 > (uint32_t)kMaxChainOps) continue;
+        if (st[j].prog.n_ops + 1 > (uint32_t)kMaxChainOps) continue;
         bool in_place = false;
-        if (gn[j].src_port.empty()) for (uint32_t ob : gn[i].out_buf) for (uint32_t ib : gn[j].in_buf) if (ob == ib) in_place = true;
+        for (const Plan::Operand& o : st[i].out) for (const Plan::Operand& q : st[j].in) if (o.space == q.space && o.index == q.index) in_place = true;
         if (in_place) continue;
-        ChainProgram pr = gn[j].prog;
-        for (uint32_t k = 0; k < gn[i].prog.n_ops; ++k) pr.ops[pr.n_ops++] = gn[i].prog.ops[k];
-        gn[i].prog = pr; gn[i].pairs = false;
-        gn[i].in_buf = gn[j].in_buf; gn[i].src_port = gn[j].src_port;
-        gn[j].absorbed = true;
+        ChainProgram pr = st[j].prog;
+        for (uint32_t k = 0; k < st[i].prog.n_ops; ++k) pr.ops[pr.n_ops++] = st[i].prog.ops[k];
+        st[i].prog = pr; st[i].pairs = false;
+        st[i].in = st[j].in;
+        folded[j] = true;
     }
+    std::vector<Plan::Step> kept;
+    for (size_t i = 0; i < n; ++i) if (!folded[i]) kept.push_back(std::move(st[i]));
+    st = std::move(kept);
 }
 
 // Device buffers of the plan (main thread): the record buffers, the silence flags and the per-call scratch of one chunk.
-static bool alloc_plan(const fw_ctx* c, Plan* plan, std::string* why) {
+static bool alloc_plan(const fw_ctx* c, Plan* plan, bool pool, std::string* why) {
     const uint32_t V = c->cfg.num_voices, F = c->max_block_frames, n_sm = plan->n_sm;
     plan->num_voices = V; plan->block_frames = F; plan->bus = c->cfg.master_bus != 0;
     DevMem& mem = plan->mem;
@@ -715,14 +734,14 @@ static bool alloc_plan(const fw_ctx* c, Plan* plan, std::string* why) {
         if (plan->bus) {
             plan->d_part[0] = mem.dev<float>((size_t)groups * n_out * Tc, false); plan->d_part[1] = mem.dev<float>((size_t)((groups + 15) / 16) * n_out * Tc, false);
         }
-        if (!plan->generic && plan->stages.size() > 1) plan->d_tmp[0] = mem.dev<float>((size_t)V * 2 * Tc, false);
-        if (!plan->generic && plan->stages.size() > 2) plan->d_tmp[1] = mem.dev<float>((size_t)V * 2 * Tc, false);
-        if (plan->generic) plan->d_pool = mem.dev<float>((size_t)plan->num_buffers * V * Tc, false);
+        for (const Plan::Step& sp : plan->steps)
+            for (const Plan::Operand& o : sp.out) if (o.space == Plan::SCRATCH && !plan->d_tmp[o.index]) plan->d_tmp[o.index] = mem.dev<float>((size_t)V * 2 * Tc, false);
+        if (pool) plan->d_pool = mem.dev<float>((size_t)plan->num_buffers * V * Tc, false);
         if (!plan->samplers.empty()) {
             plan->d_slot_of = mem.dev<uint16_t>((size_t)Kc * V);
             for (size_t i = 0; i < plan->samplers.size(); ++i) plan->d_srec.push_back(mem.dev<SmpRec>((size_t)Kc * V));
         }
-        for (auto& gn : plan->gnodes) if (gn.kind == FW_NODE_CUSTOM) { gn.custom_idx = (int)plan->d_custom_masks.size(); plan->d_custom_masks.push_back(mem.dev<uint64_t>((size_t)Kc * V)); }
+        for (auto& sp : plan->steps) if (sp.kind == Plan::Step::CUSTOM) { sp.custom_idx = (int)plan->d_custom_masks.size(); plan->d_custom_masks.push_back(mem.dev<uint64_t>((size_t)Kc * V)); }
         r.slot_of = plan->d_slot_of;
     }
     if (!mem.ok()) { *why = "device allocation failed: " + g_dev_err; return false; }
@@ -738,11 +757,12 @@ static bool lower(fw_ctx* c, const Schedule& s, Plan* plan, std::string* why) {
     if (gout.in.size() != c->n_out) { *why = "stream output channels must equal the graph_out port count on the device path"; return false; }
     plan->c_in = (uint32_t)gin.out.size(); plan->c_out = (uint32_t)gout.in.size();
     const bool bus = c->cfg.master_bus != 0;
-    if (!lower_chain(s, sm_of_node, bus, plan, why)) {
+    const bool chain = lower_chain(s, sm_of_node, bus, plan, why);
+    if (!chain) {
         if (!lower_generic(s, sm_of_node, bus, plan, why)) return false;
         fuse_generic(s, plan);
     }
-    if (!alloc_plan(c, plan, why)) return false;
+    if (!alloc_plan(c, plan, !chain, why)) return false;
     // delay cursors, reverb history cursors + tensor maps, resampler positions and plugin calls change from call to call
     plan->graphable = true;
     for (auto& st : plan->states) if (st->kind == FW_NODE_DELAY || st->kind == FW_NODE_CONV_REVERB || st->kind == FW_NODE_RESAMPLER || st->kind == FW_NODE_CUSTOM) plan->graphable = false;
@@ -1498,10 +1518,10 @@ static int run_bus_stage(fw_processor* p, Plan& pl, ChainArgs& xa, uint32_t n_ou
     return FW_PROC_OK;
 }
 
-// ---- launches of the stateful node kinds, shared by the fused-chain stages (enqueue_chunk) and the generic lowering --------------
+// ---- launches of the stateful node kinds (see enqueue_chunk) ------------------------------------------------------------------
 // C channels of every voice: row v * C + k (voice v, channel k) starts at in + row * in_pitch and at out + row * out_pitch floats.
-// A fused-chain stage passes all its channels as one block ([V][C][pitch]); the generic lowering passes every channel as a block
-// of its own (C = 1): a pool buffer [V][T] or, as input, one channel of the caller's rows (in_pitch = n_in * Tfull).
+// A step's input and output operand k resolve to block k: a fused-chain stage has one block of all its channels ([V][C][pitch]), the
+// generic lowering a block per channel (C = 1): a pool buffer [V][T] or one channel of the caller's rows (pitch = n_in * Tfull).
 struct RowBlock { const float* in; float* out; uint32_t C; uint64_t in_pitch, out_pitch; };
 static uint32_t channels_of(const RowBlock* b, uint32_t nb) { uint32_t n = 0; for (uint32_t i = 0; i < nb; ++i) n += b[i].C; return n; }
 
@@ -1560,125 +1580,6 @@ static int run_reverb(fw_processor* p, NodeDeviceState& rs, const RowBlock* b, u
             if (!FW_LAUNCH(p, 3, 2, launch_reverb(rc, p->stream, &rerr))) { if (!rerr.empty()) g_dev_err = rerr; return FW_PROC_DEVICE_ERROR; }
         }
         rs.xh_cursor += Tp;
-    }
-    return FW_PROC_OK;
-}
-
-// Generic lowering at run time: walk the scheduled nodes (compiler.rs order) over the pool [buffer][V][Tc]. Buffer reuse
-// is the reference's (compiler.rs:302-412): it is valid for any execution that respects the schedule order, and each
-// node here finishes all blocks of the chunk before the next node starts.
-static int enqueue_generic(fw_processor* p, Plan& pl, const float* d_in, float* d_out, const Chunk& ck) {
-    const uint32_t V = p->num_voices, n_in = pl.c_in, n_out = pl.c_out, T = ck.Tc;
-    const size_t BS = (size_t)V * T;  // floats per pool buffer
-    const uint64_t in_vs = (uint64_t)n_in * ck.Tfull, out_vs = (uint64_t)n_out * ck.Tfull;  // voice strides of the caller's rows
-    auto buf = [&](uint32_t b) { return pl.d_pool + (size_t)b * BS; };
-    auto caller_in = [&](size_t c) { return d_in + ck.t0 + c * (size_t)ck.Tfull; };
-    if (pl.reads_caller_rows && in_vs > 0xffffffffull) { g_dev_err = "input rows of more than 2^32 / channels frames"; return FW_PROC_BAD_ARGS; }
-    RowBlock rows[64];
-    // the node's first n channels as one-channel blocks: inputs from pool buffers or, fed by graph_in, the caller's rows; outputs to pool buffers
-    auto node_rows = [&](const Plan::GNode& gn, size_t n) -> const RowBlock* {
-        const bool caller = !gn.src_port.empty();
-        for (size_t c = 0; c < n; ++c)
-            rows[c] = RowBlock{c >= gn.in_buf.size() ? nullptr : caller ? caller_in(gn.src_port[c]) : buf(gn.in_buf[c]), buf(gn.out_buf[c]), 1, caller ? in_vs : T, T};
-        return rows;
-    };
-    auto silence_fix = [&](const Plan::GNode& gn, size_t out_ch, uint64_t test) -> bool {
-        if (gn.mask_slot < 0) return true;
-        SilenceFixArgs fa{};
-        fa.out = buf(gn.out_buf[out_ch]); fa.test = test; fa.num_voices = V; fa.frames = T; fa.block_frames = pl.block_frames; fa.mask_slot = gn.mask_slot; fa.rec = pl.rec;
-        return FW_LAUNCH(p, 1, 1, launch_silence_fix(fa, p->stream));
-    };
-    // gn.prog from pool buffers or (src_port) the caller's input rows to pool buffers or, at graph_out, the caller's output rows or the bus stage
-    auto run_prog = [&](const Plan::GNode& gn, bool gout) -> int {
-        const bool caller = !gn.src_port.empty();
-        const size_t ni = caller ? gn.src_port.size() : gn.in_buf.size(), no = gout ? n_out : gn.out_buf.size();
-        const float* in[64] = {}; float* out[64] = {};
-        for (size_t c = 0; c < ni; ++c) in[c] = caller ? caller_in(gn.src_port[c]) : buf(gn.in_buf[c]);
-        const uint64_t ivs = caller ? in_vs : T;
-        if (gout && pl.bus) { ChainArgs xa = chain_args(pl, ck, gn.prog, in, ivs, out, 0, caller); return run_bus_stage(p, pl, xa, n_out, ck, d_out + ck.t0); }
-        for (size_t c = 0; c < no; ++c) out[c] = gout ? d_out + ck.t0 + c * (size_t)ck.Tfull : buf(gn.out_buf[c]);
-        const uint64_t ovs = gout ? out_vs : T;
-        const size_t nc = std::min(ni, no);
-        for (size_t c = 0; c < (gn.pairs ? nc : 1); c += 2) {
-            ChainProgram pr = gn.prog;
-            if (gn.pairs && c + 1 == nc) pr.c_in = pr.c_out = 1;
-            if (!FW_LAUNCH(p, 1, 1, launch_chain(chain_args(pl, ck, pr, in + c, ivs, out + c, ovs, caller), false, p->stream))) return FW_PROC_DEVICE_ERROR;
-        }
-        return FW_PROC_OK;
-    };
-    const size_t N = pl.gnodes.size();
-    for (size_t i = 0; i < N; ++i) {
-        Plan::GNode& gn = pl.gnodes[i];
-        if (gn.absorbed) continue;  // runs inside the program of the node that ends its run; graph_in: every reader reads the caller's rows
-        for (size_t k = 0; k < gn.in_buf.size(); ++k)  // unconnected inputs are cleared every block (schedule.rs:310-313)
-            if (gn.in_clear[k]) { if (!FW_CUDA(launch_fill(buf(gn.in_buf[k]), BS, 0.0f, p->stream))) return FW_PROC_DEVICE_ERROR; p->launches++; }
-        // graph_in: stream channels -> pool (prepare_graph_inputs, schedule.rs:213-253); graph_out: pool -> stream channels / master bus
-        // (read_graph_outputs, schedule.rs:255-287)
-        if (i == 0 || i + 1 == N) { const int orc = run_prog(gn, i + 1 == N); if (orc != FW_PROC_OK) return orc; continue; }
-        const uint32_t zf = gn.src_port.empty() ? 0u : ck.zero_first;  // Q11 applies to the caller's rows only
-        int rc = FW_PROC_OK;
-        switch (gn.kind) {
-            case FW_NODE_DUMMY: break;  // no outputs (rejected otherwise)
-            case FW_NODE_SAMPLER:
-                rc = run_sampler(p, pl, *gn.st, pl.d_srec[gn.sampler_idx], gn.sm0, node_rows(gn, gn.out_buf.size()), (uint32_t)gn.out_buf.size(), T);
-                break;
-            case FW_NODE_VOLUME: case FW_NODE_PAN: case FW_NODE_HARD_CLIP: case FW_NODE_MONO_TO_STEREO: case FW_NODE_STEREO_TO_MONO:
-                rc = run_prog(gn, false);
-                for (size_t c = 0; rc == FW_PROC_OK && gn.mask_slot >= 0 && c < gn.out_buf.size(); ++c)  // test: the inputs output c is made of
-                    if (!silence_fix(gn, c, gn.kind == FW_NODE_STEREO_TO_MONO ? 3ull : gn.kind == FW_NODE_MONO_TO_STEREO ? 1ull : 1ull << c)) return FW_PROC_DEVICE_ERROR;
-                break;
-            case FW_NODE_SUM: {
-                const size_t no = gn.out_buf.size(), ports = no ? gn.in_buf.size() / no : 0;
-                if (ports <= 1) { rc = run_prog(gn, false); break; }  // copy (sum.rs:58-65)
-                for (size_t c = 0; c < no; ++c) {
-                    SumArgs sa{};
-                    for (size_t q = 0; q < ports; ++q) { sa.in[q] = buf(gn.in_buf[q * no + c]); sa.mask_bit[q] = (uint8_t)(q * no + c); }
-                    sa.out = buf(gn.out_buf[c]); sa.n_ports = (uint32_t)ports; sa.num_voices = V; sa.frames = T; sa.block_frames = pl.block_frames;
-                    sa.mask_slot = gn.mask_slot; sa.skip_silent = ports >= 5 ? 1u : 0u;
-                    sa.all_mask = gn.in_buf.size() >= 64 ? ~0ull : (1ull << gn.in_buf.size()) - 1ull; sa.rec = pl.rec;
-                    if (!FW_LAUNCH(p, 1, 1, launch_sum(sa, p->stream))) return FW_PROC_DEVICE_ERROR;
-                }
-                break;
-            }
-            case FW_NODE_RESAMPLER: {
-                NodeDeviceState& st = *gn.st;
-                ResamplerArgs ra{};
-                for (size_t c = 0; c < gn.out_buf.size(); ++c) ra.out[c] = buf(gn.out_buf[c]);
-                ra.out_vstride = T; ra.n_out = (uint32_t)gn.out_buf.size(); ra.num_voices = V; ra.frames = T; ra.taps = st.params->rs_taps;
-                uint32_t lg = 0; while ((1u << lg) < st.params->rs_phases) ++lg;
-                ra.phase_shift = 32 - lg;
-                ra.table = st.d_rs_table; ra.pos = st.d_rs_pos; ra.step = st.d_rs_step; ra.flags = st.d_rs_flags; ra.res = st.d_rs_res; ra.res_tab = st.cur_tab;
-                if (!FW_LAUNCH(p, 3, 2, launch_resampler(ra, st.d_rs_pos, p->stream))) return FW_PROC_DEVICE_ERROR;
-                break;
-            }
-            case FW_NODE_SVF: case FW_NODE_BIQUAD: case FW_NODE_DELAY: {
-                NodeDeviceState* st = gn.st.get();
-                rc = run_temporal(p, gn.kind == FW_NODE_DELAY ? nullptr : st, gn.kind == FW_NODE_DELAY ? st : nullptr, node_rows(gn, gn.in_buf.size()), (uint32_t)gn.in_buf.size(), T, zf);
-                break;
-            }
-            case FW_NODE_CONV_REVERB:
-                rc = run_reverb(p, *gn.st, node_rows(gn, gn.in_buf.size()), (uint32_t)gn.in_buf.size(), T, zf);
-                break;
-            case FW_NODE_CUSTOM: {  // AudioNodeProcessor::process for all voices and blocks at once (fw_node_vtable::process_device)
-                NodeDeviceState& st = *gn.st;
-                const uint32_t nb = (T + pl.block_frames - 1) / pl.block_frames;
-                uint64_t* masks = pl.d_custom_masks[gn.custom_idx];
-                if (!FW_CUDA(launch_expand_masks(pl.rec, (uint32_t)gn.mask_slot, V, nb, masks, p->stream))) return FW_PROC_DEVICE_ERROR;
-                p->launches++;
-                const float* ins[64]; float* outs[64];
-                for (size_t c = 0; c < gn.in_buf.size(); ++c) ins[c] = buf(gn.in_buf[c]);
-                for (size_t c = 0; c < gn.out_buf.size(); ++c) outs[c] = buf(gn.out_buf[c]);
-                fw_device_block blk{};
-                blk.num_voices = V; blk.num_inputs = (uint32_t)gn.in_buf.size(); blk.num_outputs = (uint32_t)gn.out_buf.size(); blk.block_frames = pl.block_frames; blk.num_blocks = nb;
-                blk.stream_status = p->cur_stream_status; blk.frames = T; blk.in_voice_stride = T; blk.out_voice_stride = T; blk.inputs = ins; blk.outputs = outs;
-                blk.in_silence_masks = masks; blk.stream_time_secs = p->cur_stream_time; blk.cuda_stream = p->stream; blk.user_cx = p->user_cx;
-                ProfScope ps(p, 1);
-                if (st.params->custom->vt.process_device(st.custom_proc, &blk) != 0) { g_dev_err = std::string("custom node '") + st.params->custom->debug_name + "': process_device failed"; return FW_PROC_DEVICE_ERROR; }
-                break;
-            }
-            default: g_dev_err = "generic lowering: unknown node kind"; return FW_PROC_DEVICE_ERROR;
-        }
-        if (rc != FW_PROC_OK) return rc;
     }
     return FW_PROC_OK;
 }
@@ -1750,7 +1651,7 @@ static bool apply_commands(fw_processor* p, Plan& pl, uint32_t b) {
 
 static constexpr uint32_t kGraphEpoch = 0x0fffffffu;  // error-word epoch of replayed chunks: always "current" (see check_device_error)
 // One chunk: control kernel + data plane over frames [ck.t0, ck.t0 + ck.Tc) of the caller's rows (ck.Tfull frames long).
-static int enqueue_chunk(fw_processor* p, Plan& pl, const float* d_in, float* d_out, uint32_t n_out, const Chunk& ck) {
+static int enqueue_chunk(fw_processor* p, Plan& pl, const float* d_in, float* d_out, const Chunk& ck) {
     const uint32_t V = p->num_voices, T = ck.Tc;
     ++p->call_epoch;
     ControlArgs ca{};
@@ -1765,32 +1666,99 @@ static int enqueue_chunk(fw_processor* p, Plan& pl, const float* d_in, float* d_
     ca.a = p->sm_a; ca.b = p->sm_b; ca.eps = p->sm_eps; ca.err_value = ((p->capturing ? kGraphEpoch : p->call_epoch) << 4) | 1u;
     if (!FW_LAUNCH(p, 0, 1, launch_control(ca, p->stream))) return FW_PROC_DEVICE_ERROR;
 
-    if (pl.generic) return enqueue_generic(p, pl, d_in, d_out, ck);
-    // ---- data plane: run the stages in order; intermediates ping-pong through [V][ch][Tc] scratch ----
-    const size_t n_stages = pl.stages.size();
-    const float* src = d_in ? d_in + ck.t0 : nullptr; uint32_t src_pitch = ck.Tfull;  // stage 0 reads the caller's rows
-    for (size_t si = 0; si < n_stages; ++si) {
-        const Plan::Stage& sg = pl.stages[si];
-        const bool last = si + 1 == n_stages;
-        float* dst = last ? d_out + ck.t0 : pl.d_tmp[si & 1];
-        const uint32_t dst_pitch = last ? ck.Tfull : T;
-        const RowBlock rows{src, dst, sg.c_out, src_pitch, dst_pitch};  // all c_out channels of a non-pointwise stage (c_in: the same or none)
-        const uint32_t zf = si == 0 ? ck.zero_first : 0u;
+    // ---- data plane: the steps in order (see Plan::Step); the generic lowering's pool buffer reuse is the reference's
+    // (compiler.rs:302-412): it is valid for any execution that respects the schedule order, and each step finishes all blocks of the
+    // chunk before the next one starts ----
+    if (pl.reads_caller_rows && (uint64_t)pl.c_in * ck.Tfull > 0xffffffffull) { g_dev_err = "input rows of more than 2^32 / channels frames"; return FW_PROC_BAD_ARGS; }
+    auto out_rows = [&](const Plan::Operand& o) -> float* {
+        return o.space == Plan::CALLER_OUT ? d_out + ck.t0 + (size_t)o.index * ck.Tfull : o.space == Plan::POOL ? pl.d_pool + (size_t)o.index * V * T : pl.d_tmp[o.index];
+    };
+    auto in_rows = [&](const Plan::Operand& o) -> const float* { return o.space == Plan::CALLER_IN ? d_in + ck.t0 + (size_t)o.index * ck.Tfull : out_rows(o); };
+    auto pitch = [&](const Plan::Operand& o) -> uint64_t {
+        if (o.space == Plan::POOL || o.space == Plan::SCRATCH) return T;
+        return o.C > 1 ? ck.Tfull : (uint64_t)(o.space == Plan::CALLER_IN ? pl.c_in : pl.c_out) * ck.Tfull;
+    };
+    RowBlock rows[64];                   // rows[k]: input operand k and output operand k
+    const float* in[64]; float* out[64];  // every input and output channel
+    for (size_t si = 0; si < pl.steps.size(); ++si) {
+        const Plan::Step& sp = pl.steps[si];
+        const uint32_t nb = (uint32_t)std::max(sp.in.size(), sp.out.size());
+        uint32_t ni = 0, no = 0; uint64_t ivs = 0, ovs = 0;  // channels and voice strides
+        in[0] = in[1] = nullptr; out[0] = out[1] = nullptr;  // chain_args reads two slots; the generic bus step has no outputs
+        for (uint32_t k = 0; k < nb; ++k) rows[k] = RowBlock{};
+        for (uint32_t k = 0; k < sp.in.size(); ++k) {
+            RowBlock& r = rows[k];
+            r.in = in_rows(sp.in[k]); r.in_pitch = pitch(sp.in[k]); r.C = sp.in[k].C; ivs = r.C * r.in_pitch;
+            for (uint32_t c = 0; c < r.C; ++c) in[ni++] = r.in + c * r.in_pitch;
+        }
+        for (uint32_t k = 0; k < sp.out.size(); ++k) {
+            RowBlock& r = rows[k];
+            r.out = out_rows(sp.out[k]); r.out_pitch = pitch(sp.out[k]); r.C = sp.out[k].C; ovs = r.C * r.out_pitch;
+            for (uint32_t c = 0; c < r.C; ++c) out[no++] = r.out + c * r.out_pitch;
+        }
+        const bool caller = !sp.in.empty() && sp.in[0].space == Plan::CALLER_IN;  // Q11 applies to the caller's rows only
+        const uint32_t zf = caller ? ck.zero_first : 0u;
+        for (uint32_t b : sp.clear) { if (!FW_CUDA(launch_fill(pl.d_pool + (size_t)b * V * T, (size_t)V * T, 0.0f, p->stream))) return FW_PROC_DEVICE_ERROR; p->launches++; }
         int rc = FW_PROC_OK;
-        switch (sg.kind) {
-            case Plan::STAGE_SAMPLER: rc = run_sampler(p, pl, *sg.node, pl.d_srec[0], sg.sampler_sm, &rows, 1, T); break;
-            case Plan::STAGE_REVERB: rc = run_reverb(p, *sg.node, &rows, 1, T, zf); break;
-            case Plan::STAGE_TEMPORAL: rc = run_temporal(p, sg.node.get(), sg.delay.get(), &rows, 1, T, zf); break;
-            case Plan::STAGE_POINTWISE: {
-                const float* in[2] = {src, src + src_pitch}; float* out[2] = {dst, dst + dst_pitch};  // staged chains read / write [V][ch][pitch]
-                ChainArgs xa = chain_args(pl, ck, sg.prog, in, (uint64_t)sg.prog.c_in * src_pitch, out, (uint64_t)sg.prog.c_out * dst_pitch, si == 0);
-                if (last && pl.bus) rc = run_bus_stage(p, pl, xa, n_out, ck, d_out + ck.t0);
-                else if (!FW_LAUNCH(p, 1, 1, launch_chain(xa, false, p->stream))) rc = FW_PROC_DEVICE_ERROR;
+        switch (sp.kind) {
+            case Plan::Step::SAMPLER: rc = run_sampler(p, pl, *sp.node, pl.d_srec[sp.sampler_idx], sp.sm0, rows, nb, T); break;
+            case Plan::Step::TEMPORAL: rc = run_temporal(p, sp.node.get(), sp.delay.get(), rows, nb, T, zf); break;
+            case Plan::Step::REVERB: rc = run_reverb(p, *sp.node, rows, nb, T, zf); break;
+            case Plan::Step::PROG:
+                if (pl.bus && si + 1 == pl.steps.size()) {
+                    ChainArgs xa = chain_args(pl, ck, sp.prog, in, ivs, out, ovs, caller);
+                    rc = run_bus_stage(p, pl, xa, pl.c_out, ck, d_out + ck.t0);
+                    break;
+                }
+                for (uint32_t c = 0, nc = std::min(ni, no); c < (sp.pairs ? nc : 1u); c += 2) {
+                    ChainProgram pr = sp.prog;
+                    if (sp.pairs && c + 1 == nc) pr.c_in = pr.c_out = 1;
+                    if (!FW_LAUNCH(p, 1, 1, launch_chain(chain_args(pl, ck, pr, in + c, ivs, out + c, ovs, caller), false, p->stream))) return FW_PROC_DEVICE_ERROR;
+                }
+                for (uint32_t c = 0; sp.mask_slot >= 0 && c < no; ++c) {  // test: the inputs output c is made of
+                    SilenceFixArgs fa{};
+                    fa.out = out[c]; fa.test = sp.prog.c_in == sp.prog.c_out ? 1ull << c : (1ull << sp.prog.c_in) - 1ull;
+                    fa.num_voices = V; fa.frames = T; fa.block_frames = pl.block_frames; fa.mask_slot = sp.mask_slot; fa.rec = pl.rec;
+                    if (!FW_LAUNCH(p, 1, 1, launch_silence_fix(fa, p->stream))) return FW_PROC_DEVICE_ERROR;
+                }
+                break;
+            case Plan::Step::SUM:
+                for (uint32_t c = 0, ports = ni / no; c < no; ++c) {
+                    SumArgs sa{};
+                    for (uint32_t q = 0; q < ports; ++q) { sa.in[q] = in[q * no + c]; sa.mask_bit[q] = (uint8_t)(q * no + c); }
+                    sa.out = out[c]; sa.n_ports = ports; sa.num_voices = V; sa.frames = T; sa.block_frames = pl.block_frames;
+                    sa.mask_slot = sp.mask_slot; sa.skip_silent = ports >= 5 ? 1u : 0u;
+                    sa.all_mask = ni >= 64 ? ~0ull : (1ull << ni) - 1ull; sa.rec = pl.rec;
+                    if (!FW_LAUNCH(p, 1, 1, launch_sum(sa, p->stream))) return FW_PROC_DEVICE_ERROR;
+                }
+                break;
+            case Plan::Step::RESAMPLER: {
+                NodeDeviceState& st = *sp.node;
+                ResamplerArgs ra{};
+                for (uint32_t c = 0; c < no; ++c) ra.out[c] = out[c];
+                ra.out_vstride = ovs; ra.n_out = no; ra.num_voices = V; ra.frames = T; ra.taps = st.params->rs_taps;
+                uint32_t lg = 0; while ((1u << lg) < st.params->rs_phases) ++lg;
+                ra.phase_shift = 32 - lg;
+                ra.table = st.d_rs_table; ra.pos = st.d_rs_pos; ra.step = st.d_rs_step; ra.flags = st.d_rs_flags; ra.res = st.d_rs_res; ra.res_tab = st.cur_tab;
+                if (!FW_LAUNCH(p, 3, 2, launch_resampler(ra, st.d_rs_pos, p->stream))) return FW_PROC_DEVICE_ERROR;
+                break;
+            }
+            case Plan::Step::CUSTOM: {  // AudioNodeProcessor::process for all voices and blocks at once (fw_node_vtable::process_device)
+                NodeDeviceState& st = *sp.node;
+                const uint32_t nblk = (T + pl.block_frames - 1) / pl.block_frames;
+                uint64_t* masks = pl.d_custom_masks[sp.custom_idx];
+                if (!FW_CUDA(launch_expand_masks(pl.rec, (uint32_t)sp.mask_slot, V, nblk, masks, p->stream))) return FW_PROC_DEVICE_ERROR;
+                p->launches++;
+                fw_device_block blk{};
+                blk.num_voices = V; blk.num_inputs = ni; blk.num_outputs = no; blk.block_frames = pl.block_frames; blk.num_blocks = nblk;
+                blk.stream_status = p->cur_stream_status; blk.frames = T; blk.in_voice_stride = T; blk.out_voice_stride = T; blk.inputs = in; blk.outputs = out;
+                blk.in_silence_masks = masks; blk.stream_time_secs = p->cur_stream_time; blk.cuda_stream = p->stream; blk.user_cx = p->user_cx;
+                ProfScope ps(p, 1);
+                if (st.params->custom->vt.process_device(st.custom_proc, &blk) != 0) { g_dev_err = std::string("custom node '") + st.params->custom->debug_name + "': process_device failed"; return FW_PROC_DEVICE_ERROR; }
                 break;
             }
         }
         if (rc != FW_PROC_OK) return rc;
-        src = dst; src_pitch = dst_pitch;
     }
     return FW_PROC_OK;
 }
@@ -1799,8 +1767,8 @@ static int enqueue_chunk(fw_processor* p, Plan& pl, const float* d_in, float* d_
 // same arguments every time: it is captured into a CUDA graph the second time it is seen and replayed from then on (one
 // cudaGraphLaunch instead of one launch per kernel; what counts for block-sized calls, where the host's launch cost exceeds the
 // kernels' run time). Programmatic-dependent-launch edges are kept by the capture.
-static int run_chunk(fw_processor* p, Plan& pl, const float* d_in, float* d_out, uint32_t n_out, const Chunk& ck, bool steady) {
-    if (!steady || !pl.graphable || p->graphs_off || p->profiling || p->world > 1 || ck.zero_first) return enqueue_chunk(p, pl, d_in, d_out, n_out, ck);
+static int run_chunk(fw_processor* p, Plan& pl, const float* d_in, float* d_out, const Chunk& ck, bool steady) {
+    if (!steady || !pl.graphable || p->graphs_off || p->profiling || p->world > 1 || ck.zero_first) return enqueue_chunk(p, pl, d_in, d_out, ck);
     const void* tabs[2 * kMaxSamplers] = {};
     for (size_t i = 0; i < pl.samplers.size() && i < (size_t)kMaxSamplers; ++i) { tabs[2 * i] = pl.samplers[i]->cur_tab; tabs[2 * i + 1] = reinterpret_cast<const void*>((uintptr_t)pl.samplers[i]->cur_n_res); }
     fw_processor::GraphEntry* e = nullptr; fw_processor::GraphEntry* lru = &p->graphs[0];
@@ -1819,12 +1787,12 @@ static int run_chunk(fw_processor* p, Plan& pl, const float* d_in, float* d_out,
         ++p->graph_replays; p->launches += e->seen;  // `seen` holds the kernel count of the captured sequence once instantiated
         return FW_PROC_OK;
     }
-    if (++e->seen < 2) return enqueue_chunk(p, pl, d_in, d_out, n_out, ck);
+    if (++e->seen < 2) return enqueue_chunk(p, pl, d_in, d_out, ck);
     // second sight: capture, instantiate, launch
     const uint64_t l0 = p->launches;
-    if (cudaStreamBeginCapture(p->stream, cudaStreamCaptureModeThreadLocal) != cudaSuccess) { cudaGetLastError(); p->graphs_off = true; return enqueue_chunk(p, pl, d_in, d_out, n_out, ck); }
+    if (cudaStreamBeginCapture(p->stream, cudaStreamCaptureModeThreadLocal) != cudaSuccess) { cudaGetLastError(); p->graphs_off = true; return enqueue_chunk(p, pl, d_in, d_out, ck); }
     p->capturing = true;
-    const int rc = enqueue_chunk(p, pl, d_in, d_out, n_out, ck);
+    const int rc = enqueue_chunk(p, pl, d_in, d_out, ck);
     p->capturing = false;
     cudaGraph_t graph = nullptr;
     const cudaError_t ce = cudaStreamEndCapture(p->stream, &graph);
@@ -1834,7 +1802,7 @@ static int run_chunk(fw_processor* p, Plan& pl, const float* d_in, float* d_out,
         cudaGetLastError();
         if (graph) cudaGraphDestroy(graph);
         e->exec = nullptr; e->plan = nullptr; p->graphs_off = true;  // capture is not available here: stay on plain launches
-        return enqueue_chunk(p, pl, d_in, d_out, n_out, ck);
+        return enqueue_chunk(p, pl, d_in, d_out, ck);
     }
     cudaGraphDestroy(graph);
     e->seen = n_launch;
@@ -1898,7 +1866,7 @@ static int proc_call(fw_processor* p, const float* d_in, float* d_out, uint32_t 
         if (p->pending_zero_first) { ck.zero_first = std::min(pl.block_frames, ck.Tc); p->pending_zero_first = false; }  // Q11
         bool steady = true;  // no sampler message rides in this chunk's control arguments (stores and uploads precede the chunk: they do not change it)
         for (auto& st : pl.samplers) if (st->cur_n_msgs) steady = false;
-        const int erc = run_chunk(p, pl, d_in, d_out, n_out, ck, steady);
+        const int erc = run_chunk(p, pl, d_in, d_out, ck, steady);
         if (erc != FW_PROC_OK) return erc;
         b = b_end;
     }
