@@ -421,7 +421,10 @@ __global__ void __launch_bounds__(kWarps * 32, kMinBlocks) chain_kernel(ChainArg
     pdl_launch_dependents();
     const uint32_t lane = threadIdx.x & 31u, warp = threadIdx.x >> 5;
     const uint32_t T = a.frames, V = a.num_voices, F = a.block_frames, NS = a.rec.n_smoothers;
-    const uint32_t c_out = a.prog.c_out;
+    // Bus variant: CTA slice z sums channels 2z and 2z + 1 of a C-channel bus (C = prog.c_out, up to kMaxBusChannels), an odd last
+    // channel alone; the channels are independent trees, so a bus over C channels is ceil(C / 2) stereo reductions on grid.z.
+    const uint32_t zc = BUS ? 2u * blockIdx.z : 0u;
+    const uint32_t c_out = BUS ? min(2u, a.prog.c_out - zc) : a.prog.c_out;
     constexpr uint32_t kTile = 32u * VEC;
     const uint32_t t = blockIdx.x * kTile + lane * VEC;
     const bool t_ok = t < T;
@@ -436,7 +439,7 @@ __global__ void __launch_bounds__(kWarps * 32, kMinBlocks) chain_kernel(ChainArg
     if (a.in_from_prev_kernel) pdl_wait();
     float x[kVPW][2][VEC];
     if (full) {
-        const float* p[2] = {a.in_ch[0] + (size_t)v0 * a.in_vstride + t, a.in_ch[CIN - 1] + (size_t)v0 * a.in_vstride + t};
+        const float* p[2] = {a.in_ch[zc] + (size_t)v0 * a.in_vstride + t, a.in_ch[zc + CIN - 1] + (size_t)v0 * a.in_vstride + t};
 #pragma unroll
         for (int j = 0; j < kVPW; ++j) {
 #pragma unroll
@@ -455,7 +458,7 @@ __global__ void __launch_bounds__(kWarps * 32, kMinBlocks) chain_kernel(ChainArg
             for (int c = 0; c < 2; ++c) {
 #pragma unroll
                 for (int i = 0; i < VEC; ++i) x[j][c][i] = 0.0f;
-                if (c < CIN && t_ok && v < V && !zero_in) VecT<VEC>::load(a.in_ch[c < CIN ? c : 0] + (size_t)v * a.in_vstride + t, x[j][c]);
+                if (c < CIN && t_ok && v < V && !zero_in) VecT<VEC>::load(a.in_ch[zc + (c < CIN ? c : 0)] + (size_t)v * a.in_vstride + t, x[j][c]);
             }
         }
     }
@@ -575,7 +578,7 @@ __global__ void __launch_bounds__(kWarps * 32, kMinBlocks) chain_kernel(ChainArg
                         for (int i = 0; i < VEC; ++i) x[j][c][i] = __fadd_rn(x[j][c][i], x[j + step][c][i]);
                 }
         // Remaining log2(kWarps) levels through shared memory; each lane owns its own frames. Producer warps
-        // arrive on a named barrier and leave; warp c (< c_out) waits, finishes channel c and stores it.
+        // arrive on a named barrier and leave; warp c (< c_out, the slice's width) waits, finishes channel zc + c and stores it.
         __shared__ float s_red[kWarps][2][32 * VEC];
 #pragma unroll
         for (int c = 0; c < 2; ++c)
@@ -598,7 +601,7 @@ __global__ void __launch_bounds__(kWarps * 32, kMinBlocks) chain_kernel(ChainArg
 #pragma unroll
                         for (int i = 0; i < VEC; ++i) p[w][i] = __fadd_rn(p[w][i], p[w + step][i]);
                     }
-            VecT<VEC>::store(a.out + ((size_t)blockIdx.y * c_out + c) * (a.bus_pitch ? a.bus_pitch : T) + t, p[0]);
+            VecT<VEC>::store(a.out + ((size_t)blockIdx.y * a.prog.c_out + zc + c) * (a.bus_pitch ? a.bus_pitch : T) + t, p[0]);
         }
     }
 }
@@ -875,7 +878,7 @@ cudaError_t launch_control(const ControlArgs& a, cudaStream_t st) {
 
 template <int VEC, int CIN, int VPW, int WARPS, int MINB>
 static cudaError_t launch_chain_v(const ChainArgs& a, bool bus, cudaStream_t st) {
-    dim3 grid((a.frames + 32 * VEC - 1) / (32 * VEC), (a.num_voices + kVPC - 1) / kVPC);
+    dim3 grid((a.frames + 32 * VEC - 1) / (32 * VEC), (a.num_voices + kVPC - 1) / kVPC, bus ? (a.prog.c_out + 1) / 2 : 1);
     if (bus) return launch_pdl(chain_kernel<VEC, CIN, true, VPW, WARPS, MINB>, grid, dim3(WARPS * 32), st, a);
     return launch_pdl(chain_kernel<VEC, CIN, false, VPW, WARPS, MINB>, grid, dim3(WARPS * 32), st, a);
 }
@@ -885,10 +888,11 @@ static cudaError_t launch_chain_t(const ChainArgs& a, bool bus, cudaStream_t st)
     return launch_chain_v<VEC, CIN, 8, 8, 2>(a, bus, st);
 }
 cudaError_t launch_chain(const ChainArgs& a, bool bus, cudaStream_t st) {
-    const uintptr_t al = reinterpret_cast<uintptr_t>(a.in_ch[0]) | reinterpret_cast<uintptr_t>(a.in_ch[1]) | reinterpret_cast<uintptr_t>(a.out_ch[0]) |
-                         reinterpret_cast<uintptr_t>(a.out_ch[1]) | reinterpret_cast<uintptr_t>(a.out) | (uintptr_t)((a.in_vstride | a.out_vstride | a.bus_pitch) * 4);
+    uintptr_t al = reinterpret_cast<uintptr_t>(a.out_ch[0]) | reinterpret_cast<uintptr_t>(a.out_ch[1]) | reinterpret_cast<uintptr_t>(a.out) |
+                   (uintptr_t)((a.in_vstride | a.out_vstride | a.bus_pitch) * 4);
+    for (const float* q : a.in_ch) al |= reinterpret_cast<uintptr_t>(q);
     const bool vec4 = (a.frames % 4 == 0) && (a.block_frames % 4 == 0) && (al % 16 == 0);
-    if (a.prog.c_in == 2) return vec4 ? launch_chain_t<4, 2>(a, bus, st) : launch_chain_t<1, 2>(a, bus, st);
+    if (a.prog.c_in >= 2) return vec4 ? launch_chain_t<4, 2>(a, bus, st) : launch_chain_t<1, 2>(a, bus, st);
     return vec4 ? launch_chain_t<4, 1>(a, bus, st) : launch_chain_t<1, 1>(a, bus, st);
 }
 uint32_t chain_voice_groups(uint32_t num_voices) { return (num_voices + kVPC - 1) / kVPC; }

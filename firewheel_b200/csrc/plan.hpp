@@ -19,6 +19,7 @@ constexpr int kMaxCtlPorts = 512;
 constexpr int kMaxSumMasks = 32;    // generic lowering: nodes whose data-plane body depends on the per-block input silence mask
 
 constexpr int kMaxSamplers = 4;     // SamplerNodes per voice graph
+constexpr int kMaxBusChannels = 8;  // graph_out channels of a master bus (7.1, the most an HDMI LPCM output carries); FW_MAX_BUS_CHANNELS
 
 enum SmStatus : uint32_t { SM_INACTIVE = 0, SM_ACTIVE = 1, SM_DEACTIVATING = 2 };   // smoother.rs:29-39
 enum RecMode : uint32_t { REC_CONST = 0, REC_CLEAR = 1, REC_CURVE = 2 };
@@ -110,7 +111,8 @@ struct ControlArgs {
 struct ChainArgs {
     // Channel c of voice v starts at in_ch[c] + v * in_vstride (floats). A staged chain reads [V][c_in][T]
     // (in_ch[c] = base + c*T, in_vstride = c_in*T); the generic lowering reads pool buffers [V][T] (in_vstride = T).
-    const float* in_ch[2]; float* out_ch[2];
+    // Only the bus variant reads more than two channels (in_ch[c_in] repeats an odd last channel); it writes no out_ch.
+    const float* in_ch[kMaxBusChannels]; float* out_ch[2];
     uint64_t in_vstride, out_vstride;
     float* out;            // bus variant only: partial bus [G][c_out][bus_pitch]
     uint32_t bus_pitch, pad3;  // floats between the rows of `out` (0: frames); the caller's bus is a column window of longer rows when a call is chunked

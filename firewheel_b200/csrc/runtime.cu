@@ -568,13 +568,15 @@ static bool lower_chain(const Schedule& s, const std::vector<int>& sm_of_node, b
     return true;
 }
 
+static_assert(kMaxBusChannels == FW_MAX_BUS_CHANNELS, "plan.hpp and the C header name the same bus limit");
+
 // Data plane, general case: the reference's own buffer assignment on device, one step per scheduled node over pool buffers. graph_in
 // copies the caller's rows to the pool, graph_out the pool to the caller's rows or the bus (prepare_graph_inputs / read_graph_outputs,
 // schedule.rs:213-287).
 static bool lower_generic(const Schedule& s, const std::vector<int>& sm_of_node, bool bus, Plan* plan, std::string* why) {
     const size_t n = s.nodes.size();
     plan->steps.clear(); plan->num_buffers = s.num_buffers;
-    if (bus && s.nodes.back().in.size() > 2) { *why = "master bus over more than 2 graph_out channels"; return false; }
+    if (bus && s.nodes.back().in.size() > (size_t)kMaxBusChannels) { *why = "master bus over more than 8 graph_out channels (FW_MAX_BUS_CHANNELS)"; return false; }
     uint32_t n_sum_masks = 0;  // nodes whose data-plane body needs the per-block input silence mask
     for (size_t i = 0; i < n; ++i) {
         const SchedNode& sn = s.nodes[i];
@@ -1447,12 +1449,15 @@ static void proc_poll(fw_processor* p) {  // processor.rs:167-206
 struct Chunk { uint32_t t0, Tc, Tfull, zero_first; };
 
 // One chain-kernel launch of `prog` over the chunk: channel c of voice v is read at in[c] + v * in_vs and written at out[c] + v * out_vs
-// (floats); an unused second channel repeats channel 0. `caller`: `in` is the caller's rows, whose first block reads as zero after a
-// schedule swap (Q11); otherwise it is the output of the preceding kernel, which the launch waits for.
+// (floats); an unused second channel repeats channel 0, and the bus stage reads all `prog.c_in` (up to kMaxBusChannels). `caller`: `in`
+// is the caller's rows, whose first block reads as zero after a schedule swap (Q11); otherwise it is the output of the preceding kernel,
+// which the launch waits for.
 static ChainArgs chain_args(const Plan& pl, const Chunk& ck, const ChainProgram& prog, const float* const* in, uint64_t in_vs, float* const* out,
                             uint64_t out_vs, bool caller) {
     ChainArgs xa{};
-    xa.in_ch[0] = in[0]; xa.in_ch[1] = in[prog.c_in > 1 ? 1 : 0]; xa.in_vstride = in_vs;
+    for (uint32_t c = 0; c < prog.c_in; ++c) xa.in_ch[c] = in[c];
+    if (prog.c_in & 1u) xa.in_ch[prog.c_in] = in[prog.c_in - 1];  // an odd last channel is read as a pair with itself
+    xa.in_vstride = in_vs;
     xa.out_ch[0] = out[0]; xa.out_ch[1] = out[prog.c_out > 1 ? 1 : 0]; xa.out_vstride = out_vs;
     xa.num_voices = pl.num_voices; xa.frames = ck.Tc; xa.block_frames = pl.block_frames; xa.zero_first_block = (caller && ck.zero_first) ? 1u : 0u;
     xa.in_from_prev_kernel = caller ? 0u : 1u; xa.rec = pl.rec; xa.prog = prog;
@@ -1684,7 +1689,7 @@ static int enqueue_chunk(fw_processor* p, Plan& pl, const float* d_in, float* d_
         const Plan::Step& sp = pl.steps[si];
         const uint32_t nb = (uint32_t)std::max(sp.in.size(), sp.out.size());
         uint32_t ni = 0, no = 0; uint64_t ivs = 0, ovs = 0;  // channels and voice strides
-        in[0] = in[1] = nullptr; out[0] = out[1] = nullptr;  // chain_args reads two slots; the generic bus step has no outputs
+        in[0] = in[1] = nullptr; out[0] = out[1] = nullptr;  // chain_args reads prog.c_in slots; the generic bus step has no outputs
         for (uint32_t k = 0; k < nb; ++k) rows[k] = RowBlock{};
         for (uint32_t k = 0; k < sp.in.size(); ++k) {
             RowBlock& r = rows[k];

@@ -15,8 +15,10 @@
  * `master_bus = 1` the graph_out channels of all voices are mixed by a balanced
  * binary tree of 2-port SumNodes (sum.rs:69-81) — level l adds neighbours
  * (2i, 2i+1); an unpaired last element is carried up unchanged (the 1-port
- * SumNode copy path, sum.rs:58-65). num_voices = 1, master_bus = 0 is exactly
- * the reference.
+ * SumNode copy path, sum.rs:58-65). Each graph_out channel has its own tree, so
+ * the bus takes 1 to FW_MAX_BUS_CHANNELS graph_out channels (mono through 7.1);
+ * the device refuses a wider bus at compile time (FW_COMPILE_UNSUPPORTED_ON_DEVICE).
+ * num_voices = 1, master_bus = 0 is exactly the reference.
  *
  * Buffer layouts (f32):
  *   interleaved in : [voice][frames][n_in]      out: [voice][frames][n_out]  (master bus: [frames][n_out])
@@ -47,6 +49,7 @@ typedef uint64_t fw_edge_id;
 #define FW_ID_DANGLING UINT64_MAX
 #define FW_ALL_VOICES UINT32_MAX
 #define FW_MAX_PORTS 64u /* node.rs:62,70; compiler.rs:202-203 */
+#define FW_MAX_BUS_CHANNELS 8u /* graph_out channels of a master bus on the device (7.1, the most HDMI LPCM carries) */
 
 typedef struct fw_ctx fw_ctx;             /* FirewheelGraphCtx   context.rs:29 */
 typedef struct fw_processor fw_processor; /* FirewheelProcessor  processor.rs:18 */
