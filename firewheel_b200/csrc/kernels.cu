@@ -80,19 +80,29 @@ __device__ __forceinline__ uint32_t sm_set_and_process(SmLocal& s, float val, ui
     return REC_CURVE;
 }
 
+__device__ __forceinline__ SmLocal sm_load(const SmDesc& d, uint32_t v) { SmLocal s; s.input = d.input[v]; s.last = d.last[v]; s.status = d.status[v]; return s; }
+__device__ __forceinline__ void sm_store(const SmDesc& d, uint32_t v, const SmLocal& s) { d.input[v] = s.input; d.last[v] = s.last; d.status[v] = s.status; }
+
 // ---- SamplerNode control (sampler.rs:331-516) ----
-struct SmpLocal { uint32_t playing, flags, res, last_play; uint64_t playhead, ls, le; };
+struct SmpLocal { uint32_t playing, flags, res; uint64_t playhead, ls, le; };
+__device__ __forceinline__ SmpLocal smp_load(const SamplerCtl& sc, uint32_t v) {
+    SmpLocal q;
+    q.playing = sc.playing[v]; q.playhead = sc.playhead[v]; q.flags = sc.loop_flags[v]; q.ls = sc.loop_start[v]; q.le = sc.loop_end[v]; q.res = sc.res[v];
+    return q;
+}
+__device__ __forceinline__ void smp_store(const SamplerCtl& sc, uint32_t v, const SmpLocal& q) {
+    sc.playing[v] = q.playing; sc.playhead[v] = q.playhead; sc.loop_flags[v] = q.flags; sc.loop_start[v] = q.ls; sc.loop_end[v] = q.le; sc.res[v] = q.res;
+}
 
 // the message drain of sampler.rs:331-414, for one voice
-__device__ __forceinline__ void smp_apply_messages(SmpLocal& q, const SamplerCtl& sc, uint32_t v) {
-    if (sc.n_msgs == 0) return;
+__device__ __forceinline__ void smp_apply_messages(SmpLocal& q, const SamplerCtl& sc, uint32_t v, const ResDesc* res_tab, uint32_t n_res) {
     for (uint32_t i = sc.msg_off[v]; i < sc.msg_off[v + 1]; ++i) {
         const SamplerMsgDev m = sc.msgs[i];
         const uint64_t loop_start_or_zero = (q.flags & 1u) ? q.ls : 0ull;
         switch (m.kind) {
             case SMSG_SET_SAMPLE:  // :333-364
                 q.res = m.a;
-                if ((q.flags & 3u) == 3u && q.res != 0 && q.res <= sc.n_res) { q.ls = 0; q.le = sc.res_tab[q.res - 1].frames; }  // update_sample :269-281
+                if ((q.flags & 3u) == 3u && q.res != 0 && q.res <= n_res) { q.ls = 0; q.le = res_tab[q.res - 1].frames; }  // update_sample :269-281
                 if (m.x) { q.playhead = loop_start_or_zero; q.playing = 0; }
                 break;
             case SMSG_PLAY: q.playing = 1; break;    // :365-371
@@ -101,7 +111,7 @@ __device__ __forceinline__ void smp_apply_messages(SmpLocal& q, const SamplerCtl
             case SMSG_SET_PLAYHEAD: q.playhead = m.x; break;  // :392-399
             default:  // SMSG_SET_LOOP :400-412
                 if (m.a == 0) { q.flags = 0; break; }
-                if (m.a == 1) { q.flags = 3u; q.ls = 0; q.le = (q.res != 0 && q.res <= sc.n_res) ? sc.res_tab[q.res - 1].frames : 0ull; }
+                if (m.a == 1) { q.flags = 3u; q.ls = 0; q.le = (q.res != 0 && q.res <= n_res) ? res_tab[q.res - 1].frames : 0ull; }
                 else { q.flags = 1u; q.ls = m.x; q.le = m.y; }
                 if (q.playhead >= q.ls && q.playhead < q.le) q.playhead = q.ls;
                 break;
@@ -130,34 +140,53 @@ __device__ __forceinline__ bool smp_step(SmpLocal& q, uint64_t len, uint32_t fra
     return true;
 }
 
+// The tables are device arrays of any size; per-voice state stays where it lives (smoothers, sampler transport: read and written in
+// place). The silence flags of the voice are n_flag_words words: word 0 (pool buffers 0-63) in a register, words 1.. — a graph of
+// more than 64 buffers — in shared memory, s_dyn[0][w - 1][thread] during the block and s_dyn[1][w - 1][thread] their value at its
+// start. When it fits (stage_tables), the table image follows them in shared memory: one parallel copy per CTA, from the kernel
+// parameters when the image travels there, instead of a chain of dependent global loads per node.
 __global__ void __launch_bounds__(128) control_kernel(const __grid_constant__ ControlArgs a) {
     pdl_launch_dependents();  // the data kernel may start loading samples now; it waits for us before reading records
+    extern __shared__ __align__(16) uint64_t s_dyn[];
+    const CtlTables& tb = a.tables;
+    const uint32_t W = tb.n_flag_words, B = blockDim.x;
+    const char* tab = static_cast<const char*>(tb.image);
+    if (a.stage_tables) {  // the tables do not change while the plan lives: copied before waiting for the previous kernel
+        uint32_t* d = reinterpret_cast<uint32_t*>(s_dyn + 2 * (size_t)(W - 1) * B);
+        const uint32_t* s = static_cast<const uint32_t*>(a.image_in_param ? static_cast<const void*>(a.image) : tb.image);
+        for (uint32_t i = threadIdx.x; i < tb.image_bytes / 4; i += B) d[i] = s[i];
+        tab = reinterpret_cast<const char*>(d);
+        __syncthreads();
+    }
     pdl_wait();               // the previous call's data kernels still read the record buffers we are about to rewrite
     const uint32_t v = blockIdx.x * blockDim.x + threadIdx.x;
     const uint32_t V = a.num_voices;
     if (v >= V) return;
-    const CtlTables& tb = a.tables;
-    const uint32_t NS = tb.n_smoothers, F = a.block_frames, NSMP = tb.n_samplers;
+    const CtlNode* const nodes = reinterpret_cast<const CtlNode*>(tab + tb.o_nodes);
+    const uint32_t* const in_port = reinterpret_cast<const uint32_t*>(tab + tb.o_in_port);
+    const uint32_t* const out_port = reinterpret_cast<const uint32_t*>(tab + tb.o_out_port);
+    const SmDesc* const smd = reinterpret_cast<const SmDesc*>(tab + tb.o_sm);
+    const SamplerCtl* const smp = reinterpret_cast<const SamplerCtl*>(tab + tb.o_smp);
+    const RsCtl* const rsc = reinterpret_cast<const RsCtl*>(tab + tb.o_rs);
+    const uint32_t NS = tb.n_smoothers, F = a.block_frames, NSMP = tb.n_samplers, MW = a.rec.n_mode_words;
     const uint32_t n_blocks = (a.frames + F - 1) / F;
     uint16_t* slot_of = const_cast<uint16_t*>(a.rec.slot_of);
+    uint64_t* const fl = s_dyn + threadIdx.x;            // word w >= 1: fl[(w - 1) * B]
+    uint64_t* const fl0 = fl + (size_t)(W - 1) * B;       // its value at the start of the block
 
-    SmLocal sm[kMaxSmoothers];
-    for (uint32_t s = 0; s < NS; ++s) { sm[s].input = tb.sm_input[s][v]; sm[s].last = tb.sm_last[s][v]; sm[s].status = tb.sm_status[s][v]; }
-    SmpLocal sl[kMaxSamplers];
-    for (uint32_t s = 0; s < NSMP; ++s) {
-        const SamplerCtl& sc = tb.smp[s];
-        sl[s].playing = sc.playing[v]; sl[s].playhead = sc.playhead[v]; sl[s].flags = sc.loop_flags[v]; sl[s].ls = sc.loop_start[v]; sl[s].le = sc.loop_end[v];
-        sl[s].res = sc.res[v]; sl[s].last_play = 0;
-        smp_apply_messages(sl[s], sc, v);
+    if (a.smp_msgs) {
+        for (uint32_t s = 0; s < NSMP; ++s) {
+            const SamplerCtl& sc = smp[s];
+            SmpLocal q = smp_load(sc, v);
+            smp_apply_messages(q, sc, v, a.smp_res_tab, a.smp_n_res);
+            smp_store(sc, v, q);
+        }
     }
-    uint64_t flags = a.flags[v];
+    uint64_t f0 = a.flags[v];
+    for (uint32_t w = 1; w < W; ++w) fl[(w - 1) * B] = a.flags[(size_t)w * V + v];
     uint64_t gout_mask = 0;
     uint32_t steady = 0xffffffffu, k = 0, last_modes = 0, slot = 0;
     bool steady_mode = false;
-    float last_vals[kMaxSmoothers];
-    for (uint32_t s = 0; s < NS; ++s) last_vals[s] = 0.0f;
-    uint64_t last_sum_mask[kMaxSumMasks];
-    for (int s = 0; s < kMaxSumMasks; ++s) last_sum_mask[s] = 0;
 
     for (; k < n_blocks; ++k) {
         const uint32_t frames = min(F, a.frames - k * F);
@@ -165,14 +194,23 @@ __global__ void __launch_bounds__(128) control_kernel(const __grid_constant__ Co
             // Nothing but sampler playheads moves. The block replays the steady record unless a non-looping sample
             // reaches its end in it (sampler.rs:486-513), which starts a new transient.
             bool evt = false;
-            for (uint32_t s = 0; s < NSMP; ++s)
-                if (sl[s].last_play && !(sl[s].flags & 1u) && sl[s].playhead + frames > tb.smp[s].res_tab[sl[s].res - 1].frames) evt = true;
+            for (uint32_t s = 0; s < NSMP; ++s) {
+                const SamplerCtl& sc = smp[s];
+                if (!sc.last_play[v]) continue;
+                const uint32_t res = sc.res[v];
+                if (!(sc.loop_flags[v] & 1u) && sc.playhead[v] + frames > a.smp_res_tab[res - 1].frames) evt = true;
+            }
             if (!evt) {
                 for (uint32_t s = 0; s < NSMP; ++s) {
+                    const SamplerCtl& sc = smp[s];
                     SmpRec r; r.p0 = 0; r.first = 0; r.mode = SMP_CLEAR;
-                    bool dummy = false;
-                    if (sl[s].last_play) smp_step(sl[s], tb.smp[s].res_tab[sl[s].res - 1].frames, frames, &r, dummy);
-                    tb.smp[s].rec[(size_t)k * V + v] = r;
+                    if (sc.last_play[v]) {
+                        SmpLocal q = smp_load(sc, v);
+                        bool dummy = false;
+                        smp_step(q, a.smp_res_tab[q.res - 1].frames, frames, &r, dummy);
+                        sc.playhead[v] = q.playhead;  // the only field a replayed block moves
+                    }
+                    sc.rec[(size_t)k * V + v] = r;
                 }
                 slot_of[(size_t)k * V + v] = (uint16_t)slot;
                 continue;
@@ -181,87 +219,118 @@ __global__ void __launch_bounds__(128) control_kernel(const __grid_constant__ Co
         }
         if (slot >= a.rec.kt_max) { *a.rec.error = a.err_value; break; }
         bool changed = false;  // smoother / sampler transport state moved during this block
-        const uint64_t flags0 = flags;  // the block is a pure function of (flags, that state): equal at both ends => it replays
-        uint32_t modes = 0;
+        const uint64_t f0_start = f0;  // the block is a pure function of (flags, that state): equal at both ends => it replays
+        for (uint32_t w = 1; w < W; ++w) fl0[(w - 1) * B] = fl[(w - 1) * B];
+        // Mode words of this record: smoothers are numbered in schedule order, so the walk meets them word by word and each word
+        // is stored once, when the walk has moved past it.
+        uint32_t mw = 0, mword = 0, mor = 0;
+        uint32_t* const modes = a.rec.modes + (size_t)slot * MW * V + v;
+        auto put_mode = [&](int32_t s, uint32_t m) {
+            const uint32_t w = (uint32_t)s / kModesPerWord;
+            for (; mw < w; ++mw) { modes[(size_t)mw * V] = mword; mor |= mword; mword = 0; }
+            mword |= m << (2 * ((uint32_t)s % kModesPerWord));
+        };
+        auto put_val = [&](int32_t s, float cv) {
+            a.rec.vals[((size_t)slot * NS + s) * V + v] = cv;
+            a.rec.st_vals[(size_t)s * V + v] = cv;  // the last value written is the steady record's
+        };
+        auto curve_of = [&](int32_t s) { return a.rec.curves + (((size_t)slot * NS + s) * V + v) * F; };
         for (uint32_t n = 0; n < tb.n_nodes; ++n) {
-            const CtlNode nd = tb.nodes[n];
+            const CtlNode nd = nodes[n];
             uint64_t in_mask = 0;
             for (uint32_t i = 0; i < nd.n_in; ++i) {  // schedule.rs:305-320
-                const uint64_t bit = 1ull << tb.in_buf[nd.in_off + i];
-                if (tb.in_clear[nd.in_off + i]) flags |= bit;
-                if (flags & bit) in_mask |= 1ull << i;
+                const uint32_t pb = in_port[nd.in_off + i], b = pb & ~kPortClear;
+                const uint64_t bit = 1ull << (b & 63u);
+                bool set;
+                if (b < 64u) { if (pb & kPortClear) f0 |= bit; set = (f0 & bit) != 0; }
+                else { uint64_t& word = fl[((b >> 6) - 1) * B]; if (pb & kPortClear) word |= bit; set = (word & bit) != 0; }
+                if (set) in_mask |= 1ull << i;
             }
-            if (nd.mask_slot) { a.rec.sum_masks[((size_t)slot * a.rec.n_sum_masks + (nd.mask_slot - 1)) * V + v] = in_mask; last_sum_mask[nd.mask_slot - 1] = in_mask; }
+            if (nd.mask_slot) {
+                a.rec.sum_masks[((size_t)slot * a.rec.n_sum_masks + (nd.mask_slot - 1)) * V + v] = in_mask;
+                a.rec.st_sum_masks[(size_t)(nd.mask_slot - 1) * V + v] = in_mask;  // the last mask written is the steady record's
+            }
             uint64_t out_mask = 0;  // processor.rs:233 NONE_SILENT
             switch (nd.kind) {
                 case FW_NODE_VOLUME: {
-                    SmLocal& s = sm[nd.sm0];
-                    const float g = tb.sm_target[nd.sm0][v];  // volume.rs:92
+                    const SmDesc d = smd[nd.sm0];
+                    SmLocal s = sm_load(d, v);
+                    bool ch = false;
+                    const float g = d.target[v];  // volume.rs:92
                     if (all_channels_silent(in_mask, nd.n_in)) {  // volume.rs:94-100
-                        sm_reset(s, g, changed);
-                        modes |= REC_CLEAR << (2 * nd.sm0);
+                        sm_reset(s, g, ch);
+                        put_mode(nd.sm0, REC_CLEAR);
                         out_mask = all_silent_mask(nd.n_out);
                     } else {
                         float cv; bool smoothing;
-                        float* curve = a.rec.curves + ((size_t)(slot * NS + nd.sm0) * V + v) * F;
-                        uint32_t m = sm_set_and_process(s, g, frames, a.a, a.b, a.eps, curve, &cv, &smoothing, changed);
+                        uint32_t m = sm_set_and_process(s, g, frames, a.a, a.b, a.eps, curve_of(nd.sm0), &cv, &smoothing, ch);
                         if (!smoothing && cv < 0.00001f) {  // volume.rs:104-108
                             m = REC_CLEAR; out_mask = all_silent_mask(nd.n_out);
                         } else {
                             out_mask = in_mask;  // volume.rs:110
                         }
-                        modes |= m << (2 * nd.sm0);
-                        a.rec.vals[(size_t)(slot * NS + nd.sm0) * V + v] = cv; last_vals[nd.sm0] = cv;
+                        put_mode(nd.sm0, m);
+                        put_val(nd.sm0, cv);
                     }
+                    if (ch) { sm_store(d, v, s); changed = true; }
                     break;
                 }
                 case FW_NODE_PAN: {
-                    const float gl = tb.sm_target[nd.sm0][v], gr = tb.sm_target[nd.sm1][v];
+                    const SmDesc dl = smd[nd.sm0], dr = smd[nd.sm1];
+                    SmLocal sl = sm_load(dl, v), sr = sm_load(dr, v);
+                    bool chl = false, chr = false;
+                    const float gl = dl.target[v], gr = dr.target[v];
                     if (all_channels_silent(in_mask, nd.n_in)) {
-                        sm_reset(sm[nd.sm0], gl, changed); sm_reset(sm[nd.sm1], gr, changed);
-                        modes |= (REC_CLEAR << (2 * nd.sm0)) | (REC_CLEAR << (2 * nd.sm1));
+                        sm_reset(sl, gl, chl); sm_reset(sr, gr, chr);
+                        put_mode(nd.sm0, REC_CLEAR); put_mode(nd.sm1, REC_CLEAR);
                         out_mask = all_silent_mask(nd.n_out);
                     } else {
                         float cv; bool smoothing;
-                        uint32_t m = sm_set_and_process(sm[nd.sm0], gl, frames, a.a, a.b, a.eps,
-                                                        a.rec.curves + ((size_t)(slot * NS + nd.sm0) * V + v) * F, &cv, &smoothing, changed);
-                        modes |= m << (2 * nd.sm0);
-                        a.rec.vals[(size_t)(slot * NS + nd.sm0) * V + v] = cv; last_vals[nd.sm0] = cv;
-                        m = sm_set_and_process(sm[nd.sm1], gr, frames, a.a, a.b, a.eps,
-                                               a.rec.curves + ((size_t)(slot * NS + nd.sm1) * V + v) * F, &cv, &smoothing, changed);
-                        modes |= m << (2 * nd.sm1);
-                        a.rec.vals[(size_t)(slot * NS + nd.sm1) * V + v] = cv; last_vals[nd.sm1] = cv;
+                        uint32_t m = sm_set_and_process(sl, gl, frames, a.a, a.b, a.eps, curve_of(nd.sm0), &cv, &smoothing, chl);
+                        put_mode(nd.sm0, m);
+                        put_val(nd.sm0, cv);
+                        m = sm_set_and_process(sr, gr, frames, a.a, a.b, a.eps, curve_of(nd.sm1), &cv, &smoothing, chr);
+                        put_mode(nd.sm1, m);
+                        put_val(nd.sm1, cv);
                         out_mask = in_mask;
                     }
+                    if (chl) { sm_store(dl, v, sl); changed = true; }
+                    if (chr) { sm_store(dr, v, sr); changed = true; }
                     break;
                 }
                 case FW_NODE_SAMPLER: {  // sampler.rs:416-559
-                    SmpLocal& q = sl[nd.sm1];
-                    const SamplerCtl& sc = tb.smp[nd.sm1];
+                    const SamplerCtl& sc = smp[nd.sm1];
+                    SmpLocal q = smp_load(sc, v);
                     SmpRec r; r.p0 = 0; r.first = 0; r.mode = SMP_CLEAR;
                     bool play = false; uint32_t sch = 0;
-                    if (q.res != 0 && q.res <= sc.n_res && q.playing) {
-                        const ResDesc rd = sc.res_tab[q.res - 1];
+                    if (q.res != 0 && q.res <= a.smp_n_res && q.playing) {
+                        const ResDesc rd = a.smp_res_tab[q.res - 1];
                         sch = rd.channels;
+                        const SmDesc d = smd[nd.sm0];
+                        SmLocal s = sm_load(d, v);
+                        bool ch = false;
                         float cv; bool smoothing;
-                        float* curve = a.rec.curves + ((size_t)(slot * NS + nd.sm0) * V + v) * F;
-                        const uint32_t m = sm_set_and_process(sm[nd.sm0], tb.sm_target[nd.sm0][v], frames, a.a, a.b, a.eps, curve, &cv, &smoothing, changed);  // :432-433
-                        modes |= m << (2 * nd.sm0);
-                        a.rec.vals[(size_t)(slot * NS + nd.sm0) * V + v] = cv; last_vals[nd.sm0] = cv;
-                        if (smoothing || !(cv < 0.00001f)) play = smp_step(q, rd.frames, frames, &r, changed);  // :437-443 muted => clear, playhead stays
+                        const uint32_t m = sm_set_and_process(s, d.target[v], frames, a.a, a.b, a.eps, curve_of(nd.sm0), &cv, &smoothing, ch);  // :432-433
+                        if (ch) { sm_store(d, v, s); changed = true; }
+                        put_mode(nd.sm0, m);
+                        put_val(nd.sm0, cv);
+                        if (smoothing || !(cv < 0.00001f)) {  // :437-443 muted => clear, playhead stays
+                            play = smp_step(q, rd.frames, frames, &r, changed);
+                            smp_store(sc, v, q);
+                        }
                     }
                     if (!play) out_mask = all_silent_mask(nd.n_out);
                     else if (nd.n_out > sch && !(nd.n_out == 2 && sch == 1))  // :545-559: channels past the sample's are zeroed and flagged
                         out_mask = all_silent_mask(nd.n_out) & ~all_silent_mask(sch);
-                    q.last_play = play ? 1u : 0u;
+                    sc.last_play[v] = play ? 1u : 0u;
                     sc.rec[(size_t)k * V + v] = r;
                     break;
                 }
                 case FW_NODE_RESAMPLER: {  // spec ours: cleared + flagged when not playing / no resource; surplus channels as the sampler's
-                    const RsCtl& rc = tb.rs[nd.sm1];
+                    const RsCtl rc = rsc[nd.sm1];
                     const uint32_t r = rc.res[v];
-                    if (!(rc.flags[v] & 1u) || r == 0 || r > rc.n_res) out_mask = all_silent_mask(nd.n_out);
-                    else { const uint32_t sch = rc.res_tab[r - 1].channels; if (nd.n_out > sch && !(nd.n_out == 2 && sch == 1)) out_mask = all_silent_mask(nd.n_out) & ~all_silent_mask(sch); }
+                    if (!(rc.flags[v] & 1u) || r == 0 || r > a.rs_n_res) out_mask = all_silent_mask(nd.n_out);
+                    else { const uint32_t sch = a.rs_res_tab[r - 1].channels; if (nd.n_out > sch && !(nd.n_out == 2 && sch == 1)) out_mask = all_silent_mask(nd.n_out) & ~all_silent_mask(sch); }
                     break;
                 }
                 case FW_NODE_SUM:  // sum.rs:52-65; the unrolled / generic sums never write the mask (Q7)
@@ -285,14 +354,19 @@ __global__ void __launch_bounds__(128) control_kernel(const __grid_constant__ Co
             }
             if (n + 1 == tb.n_nodes) gout_mask = in_mask;  // graph_out is scheduled last (compiler.rs:291)
             for (uint32_t i = 0; i < nd.n_out; ++i) {  // schedule.rs:338-341
-                const uint64_t bit = 1ull << tb.out_buf[nd.out_off + i];
-                flags = (out_mask >> i) & 1ull ? (flags | bit) : (flags & ~bit);
+                const uint32_t b = out_port[nd.out_off + i];
+                const uint64_t bit = 1ull << (b & 63u);
+                const bool set = (out_mask >> i) & 1ull;
+                if (b < 64u) f0 = set ? (f0 | bit) : (f0 & ~bit);
+                else { uint64_t& word = fl[((b >> 6) - 1) * B]; word = set ? (word | bit) : (word & ~bit); }
             }
         }
-        a.rec.modes[(size_t)slot * V + v] = modes;
-        last_modes = modes;
+        for (; mw < MW; ++mw) { modes[(size_t)mw * V] = mword; mor |= mword; mword = 0; }
+        last_modes = mor;
         if (slot_of) slot_of[(size_t)k * V + v] = (uint16_t)slot;
-        if (!changed && flags == flags0) {  // nothing moved: later blocks replay this record
+        bool same = f0 == f0_start;
+        for (uint32_t w = 1; w < W; ++w) same = same && fl0[(w - 1) * B] == fl[(w - 1) * B];
+        if (!changed && same) {  // nothing moved: later blocks replay this record
             steady = k;
             if (NSMP == 0) break;
             steady_mode = true;
@@ -302,16 +376,10 @@ __global__ void __launch_bounds__(128) control_kernel(const __grid_constant__ Co
     }
     if (steady == 0xffffffffu) steady = (k == 0 ? 0 : min(k, n_blocks) - 1);
     a.rec.steady_k[v] = steady;
-    a.rec.st_modes[v] = last_modes;  // the record of block `steady`, flattened
-    for (uint32_t s = 0; s < NS; ++s) a.rec.st_vals[(size_t)s * V + v] = last_vals[s];
-    for (uint32_t s = 0; s < a.rec.n_sum_masks; ++s) a.rec.st_sum_masks[(size_t)s * V + v] = last_sum_mask[s];
+    a.rec.st_modes[v] = last_modes;  // the record of block `steady`: any smoother not REC_CONST
     a.rec.gout_mask[v] = gout_mask;
-    for (uint32_t s = 0; s < NS; ++s) { tb.sm_input[s][v] = sm[s].input; tb.sm_last[s][v] = sm[s].last; tb.sm_status[s][v] = sm[s].status; }
-    for (uint32_t s = 0; s < NSMP; ++s) {
-        const SamplerCtl& sc = tb.smp[s];
-        sc.playing[v] = sl[s].playing; sc.playhead[v] = sl[s].playhead; sc.loop_flags[v] = sl[s].flags; sc.loop_start[v] = sl[s].ls; sc.loop_end[v] = sl[s].le; sc.res[v] = sl[s].res;
-    }
-    a.flags[v] = flags;
+    a.flags[v] = f0;
+    for (uint32_t w = 1; w < W; ++w) a.flags[(size_t)w * V + v] = fl[(w - 1) * B];
 }
 
 // =============================================================================================
@@ -344,8 +412,14 @@ __device__ __forceinline__ uint32_t rec_slot(const Records& r, uint32_t v, uint3
     return min(k, r.steady_k[v]);
 }
 
+// mode of smoother s in a record: modes points at word 0 of the (slot, voice), words are V apart
+__device__ __forceinline__ uint32_t rec_mode(const uint32_t* modes, uint32_t V, uint32_t s) {
+    return (modes[(size_t)(s / kModesPerWord) * V] >> (2 * (s % kModesPerWord))) & 3u;
+}
+
 struct RecView {  // per-voice record access, either from the CTA's smem stage or straight from global
-    uint32_t kk, modes;
+    uint32_t kk;
+    const uint32_t* modes;  // word w of the record: modes[w * V]
     const float* vals;  // vals[s * stride]
     uint32_t stride;
 };
@@ -358,7 +432,7 @@ __device__ __forceinline__ void apply_chain(const ChainArgs& a, const RecView& r
         const ChainOp op = a.prog.ops[o];
         switch (op.kind) {
             case OP_GAIN: {  // volume.rs:116-143: out = in * gain[i] (both channels share the curve)
-                const uint32_t m = (r.modes >> (2 * op.sm0)) & 3u;
+                const uint32_t m = rec_mode(r.modes, V, (uint32_t)op.sm0);
                 if (m == REC_CLEAR) {
 #pragma unroll
                     for (int i = 0; i < VEC; ++i) { x[0][i] = 0.0f; x[1][i] = 0.0f; }
@@ -375,7 +449,7 @@ __device__ __forceinline__ void apply_chain(const ChainArgs& a, const RecView& r
                 break;
             }
             case OP_PAN: {
-                const uint32_t m0 = (r.modes >> (2 * op.sm0)) & 3u, m1 = (r.modes >> (2 * op.sm1)) & 3u;
+                const uint32_t m0 = rec_mode(r.modes, V, (uint32_t)op.sm0), m1 = rec_mode(r.modes, V, (uint32_t)op.sm1);
                 if (m0 == REC_CLEAR) {
 #pragma unroll
                     for (int i = 0; i < VEC; ++i) { x[0][i] = 0.0f; x[1][i] = 0.0f; }
@@ -420,7 +494,7 @@ __global__ void __launch_bounds__(kWarps * 32, kMinBlocks) chain_kernel(ChainArg
     static_assert(kVPW * kWarps == kVPC, "a CTA owns 64 voices");
     pdl_launch_dependents();
     const uint32_t lane = threadIdx.x & 31u, warp = threadIdx.x >> 5;
-    const uint32_t T = a.frames, V = a.num_voices, F = a.block_frames, NS = a.rec.n_smoothers;
+    const uint32_t T = a.frames, V = a.num_voices, F = a.block_frames, NS = a.rec.n_smoothers, MW = a.rec.n_mode_words;
     // Bus variant: CTA slice z sums channels 2z and 2z + 1 of a C-channel bus (C = prog.c_out, up to kMaxBusChannels), an odd last
     // channel alone; the channels are independent trees, so a bus over C channels is ceil(C / 2) stereo reductions on grid.z.
     const uint32_t zc = BUS ? 2u * blockIdx.z : 0u;
@@ -468,16 +542,17 @@ __global__ void __launch_bounds__(kWarps * 32, kMinBlocks) chain_kernel(ChainArg
     // ---- per-warp record staging: one independent load per voice, no CTA-wide barrier ---------------
     // Steady voices (block >= steady_k[v], all smoothers REC_CONST) take the fast path; a warp that owns any
     // transient / CLEAR / CURVE voice, or a tile that straddles block boundaries, takes the generic path.
-    __shared__ float s_wv[kWarps][kMaxSmoothers][kVPW];
+    // Only the program's own smoothers are staged, at program-local indices.
+    __shared__ float s_wv[kWarps][kMaxProgSmoothers][kVPW];
     const bool cta_uniform = (F % kTile) == 0u;
     bool warp_fast = false;
     if (cta_uniform) {
         const uint32_t kb = (blockIdx.x * kTile) / F;
         uint32_t special = 0;
         if (lane < kVPW && v0 + lane < V) special = (kb < a.rec.steady_k[v0 + lane]) || (a.rec.st_modes[v0 + lane] != 0u);
-        for (uint32_t i = lane; i < NS * kVPW; i += 32u) {
+        for (uint32_t i = lane; i < a.prog.n_sm * kVPW; i += 32u) {
             const uint32_t s = i / kVPW, j = i % kVPW;
-            s_wv[warp][s][j] = (v0 + j < V) ? a.rec.st_vals[(size_t)s * V + v0 + j] : 0.0f;
+            s_wv[warp][s][j] = (v0 + j < V) ? a.rec.st_vals[(size_t)a.prog.sm[s] * V + v0 + j] : 0.0f;
         }
         warp_fast = !__any_sync(0xffffffffu, special);
         __syncwarp();
@@ -491,14 +566,14 @@ __global__ void __launch_bounds__(kWarps * 32, kMinBlocks) chain_kernel(ChainArg
             if (op.kind == OP_GAIN) {  // volume.rs:123-126
 #pragma unroll
                 for (int j = 0; j < kVPW; ++j) {
-                    const float g = s_wv[warp][op.sm0][j];
+                    const float g = s_wv[warp][op.l0][j];
 #pragma unroll
                     for (int i = 0; i < VEC; ++i) { x[j][0][i] = __fmul_rn(x[j][0][i], g); x[j][1][i] = __fmul_rn(x[j][1][i], g); }
                 }
             } else if (op.kind == OP_PAN) {
 #pragma unroll
                 for (int j = 0; j < kVPW; ++j) {
-                    const float gl = s_wv[warp][op.sm0][j], gr = s_wv[warp][op.sm1][j];
+                    const float gl = s_wv[warp][op.l0][j], gr = s_wv[warp][op.l1][j];
 #pragma unroll
                     for (int i = 0; i < VEC; ++i) { x[j][0][i] = __fmul_rn(x[j][0][i], gl); x[j][1][i] = __fmul_rn(x[j][1][i], gr); }
                 }
@@ -534,7 +609,7 @@ __global__ void __launch_bounds__(kWarps * 32, kMinBlocks) chain_kernel(ChainArg
             const uint32_t v = v0 + j;
             if (v < V && t_ok) {
                 RecView r;
-                r.kk = rec_slot(a.rec, v, k, V); r.modes = a.rec.modes[(size_t)r.kk * V + v];
+                r.kk = rec_slot(a.rec, v, k, V); r.modes = a.rec.modes + (size_t)r.kk * MW * V + v;
                 r.vals = a.rec.vals + (size_t)r.kk * NS * V + v; r.stride = V;
                 apply_chain<VEC>(a, r, v, t_in_block, xs[j]);
             }
@@ -703,7 +778,7 @@ __global__ void __launch_bounds__(128) sampler_kernel(const __grid_constant__ Sa
         else { VecT<VEC>::store(dst, y); return; }                    // :552-558 zeroed (and flagged by the control kernel)
     }
     const uint32_t kk = rec_slot(a.rec, v, k, V), NS = a.rec.n_smoothers;
-    const uint32_t m = (a.rec.modes[(size_t)kk * V + v] >> (2 * a.sm)) & 3u;
+    const uint32_t m = rec_mode(a.rec.modes + (size_t)kk * a.rec.n_mode_words * V + v, V, (uint32_t)a.sm);
     float g[VEC];
     if (m == REC_CURVE) {
 #pragma unroll
@@ -861,19 +936,45 @@ static inline unsigned grid_for(size_t n) { size_t b = (n + 255) / 256; return (
 // All three per-call kernels are launched with programmatic stream serialization: each begins with
 // griddepcontrol.launch_dependents and reads its predecessor's results only after griddepcontrol.wait.
 template <class... KArgs, class... Args>
-static cudaError_t launch_pdl(void (*kernel)(KArgs...), dim3 grid, dim3 block, cudaStream_t st, Args&&... args) {
+static cudaError_t launch_pdl_smem(void (*kernel)(KArgs...), dim3 grid, dim3 block, size_t smem, cudaStream_t st, Args&&... args) {
     cudaLaunchConfig_t cfg{};
-    cfg.gridDim = grid; cfg.blockDim = block; cfg.dynamicSmemBytes = 0; cfg.stream = st;
+    cfg.gridDim = grid; cfg.blockDim = block; cfg.dynamicSmemBytes = smem; cfg.stream = st;
     cudaLaunchAttribute attr[1];
     attr[0].id = cudaLaunchAttributeProgrammaticStreamSerialization;
     attr[0].val.programmaticStreamSerializationAllowed = 1;
     cfg.attrs = attr; cfg.numAttrs = 1;
     return cudaLaunchKernelEx(&cfg, kernel, std::forward<Args>(args)...);
 }
+template <class... KArgs, class... Args>
+static cudaError_t launch_pdl(void (*kernel)(KArgs...), dim3 grid, dim3 block, cudaStream_t st, Args&&... args) {
+    return launch_pdl_smem(kernel, grid, block, 0, st, std::forward<Args>(args)...);
+}
 
-cudaError_t launch_control(const ControlArgs& a, cudaStream_t st) {
-    const uint32_t threads = 128, blocks = (a.num_voices + threads - 1) / threads;
-    return launch_pdl(control_kernel, dim3(blocks), dim3(threads), st, a);
+// Threads per CTA of the control kernel: 128 while the shared-memory flags of a voice (two copies of words 1 .. n_flag_words - 1) fit in
+// 48 KB for all of them, else fewer, up to the device's opt-in limit; 0 when not even one voice fits.
+uint32_t control_threads(uint32_t n_flag_words, int device) {
+    const size_t per_thread = 2 * sizeof(uint64_t) * (size_t)(n_flag_words - 1);
+    if (per_thread * 128 <= 48 * 1024) return 128;
+    int optin = 0;
+    if (cudaDeviceGetAttribute(&optin, cudaDevAttrMaxSharedMemoryPerBlockOptin, device) != cudaSuccess) return 0;
+    uint32_t t = 64;
+    while (t > 0 && per_thread * t > (size_t)optin) t >>= 1;
+    return t;
+}
+cudaError_t launch_control(ControlArgs a, cudaStream_t st) {
+    int device = 0;
+    cudaGetDevice(&device);
+    const CtlTables& tb = a.tables;
+    const uint32_t threads = control_threads(tb.n_flag_words, device);
+    if (threads == 0) return cudaErrorInvalidValue;
+    size_t smem = 2 * sizeof(uint64_t) * (size_t)(tb.n_flag_words - 1) * threads;
+    a.stage_tables = smem + tb.image_bytes <= 48 * 1024 ? 1u : 0u;  // larger tables are read from global memory, where L1 keeps them after the first block
+    if (a.stage_tables) smem += tb.image_bytes;
+    if (smem > 48 * 1024) {
+        const cudaError_t e = cudaFuncSetAttribute(control_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
+        if (e != cudaSuccess) return e;
+    }
+    return launch_pdl_smem(control_kernel, dim3((a.num_voices + threads - 1) / threads), dim3(threads), smem, st, a);
 }
 
 template <int VEC, int CIN, int VPW, int WARPS, int MINB>

@@ -10,7 +10,8 @@
 #include "plan.hpp"
 
 namespace fw {
-cudaError_t launch_control(const ControlArgs& a, cudaStream_t st);
+cudaError_t launch_control(ControlArgs a, cudaStream_t st);
+uint32_t control_threads(uint32_t n_flag_words, int device);  // CTA size of the control kernel, 0: the flags of one voice do not fit
 cudaError_t launch_chain(const ChainArgs& a, bool bus, cudaStream_t st);
 uint32_t chain_voice_groups(uint32_t num_voices);  // partial buses produced by the bus variant
 cudaError_t launch_sum(const SumArgs& a, cudaStream_t st);

@@ -1,8 +1,8 @@
 // plan.hpp — PODs shared by the host lowering and the sm_90a kernels.
 //
 // A compiled voice graph is lowered to
-//   * CtlTables  — the schedule as the CONTROL kernel sees it: one thread per voice walks the
-//                  scheduled nodes per block and restates the reference's per-block control logic
+//   * CtlTables  — the schedule as the CONTROL kernel sees it (device arrays built once per plan): one thread per
+//                  voice walks the scheduled nodes per block and restates the reference's per-block control logic
 //                  (silence flags schedule.rs:305-341, ParamSmoother state machine smoother.rs:115-194,
 //                  gain's early-outs volume.rs:94-108), emitting one small record per (voice, block);
 //   * ChainProgram — the DATA plane: a linear chain of pointwise node bodies fused into one
@@ -13,26 +13,28 @@
 namespace fw {
 
 constexpr int kMaxChainOps = 16;
-constexpr int kMaxSmoothers = 16;   // 2 mode bits each in a 32-bit record word
-constexpr int kMaxCtlNodes = 64;
-constexpr int kMaxCtlPorts = 512;
-constexpr int kMaxSumMasks = 32;    // generic lowering: nodes whose data-plane body depends on the per-block input silence mask
+constexpr int kMaxProgSmoothers = 16;  // distinct smoothers one ChainProgram reads (the chain kernel stages them in shared memory)
+constexpr int kModesPerWord = 16;      // 2 mode bits per smoother in a 32-bit record word
 
-constexpr int kMaxSamplers = 4;     // SamplerNodes per voice graph
 constexpr int kMaxBusChannels = 8;  // graph_out channels of a master bus (7.1, the most an HDMI LPCM output carries); FW_MAX_BUS_CHANNELS
 
 enum SmStatus : uint32_t { SM_INACTIVE = 0, SM_ACTIVE = 1, SM_DEACTIVATING = 2 };   // smoother.rs:29-39
 enum RecMode : uint32_t { REC_CONST = 0, REC_CLEAR = 1, REC_CURVE = 2 };
 
 enum ChainOpKind : uint32_t { OP_GAIN = 0, OP_PAN = 1, OP_CLIP = 2, OP_M2S = 3, OP_S2M = 4 };
-struct ChainOp { uint32_t kind; int32_t sm0, sm1; float f0; };
-struct ChainProgram { uint32_t n_ops, c_in, c_out, pad; ChainOp ops[kMaxChainOps]; };
+// sm0 / sm1: the plan's smoother indices (-1: none); l0 / l1: the same smoothers' program-local indices (ChainProgram::sm[l] = sm),
+// where the chain kernel stages the steady values
+struct ChainOp { uint32_t kind; int32_t sm0, sm1; float f0; int32_t l0, l1; };
+struct ChainProgram { uint32_t n_ops, c_in, c_out, n_sm; ChainOp ops[kMaxChainOps]; int32_t sm[kMaxProgSmoothers]; };
 
 struct CtlNode {
-    uint8_t kind, n_in, n_out, mask_slot;  // mask_slot: 1 + index into Records::sum_masks, 0 = none
-    uint16_t in_off, out_off;   // into in_buf / in_clear / out_buf
-    int16_t sm0, sm1;           // smoother indices (-1: none); SamplerNode: sm1 = index into CtlTables::smp; custom node: sm0 = fw_out_silence_rule
+    uint8_t kind, n_in, n_out, pad;
+    uint32_t in_off, out_off;   // into CtlTables::in_port / out_port
+    int32_t sm0, sm1;           // smoother indices (-1: none); SamplerNode / ResamplerNode: sm1 = index into CtlTables::smp / rs; custom node: sm0 = fw_out_silence_rule
+    uint32_t mask_slot;         // 1 + index into Records::sum_masks, 0 = none
 };
+// One smoother: its per-voice state (SoA over voices, owned by the node's device state) and its target parameter
+struct SmDesc { float* input; float* last; uint32_t* status; const float* target; };
 
 // ---- SamplerNode (sampler.rs:283-560) on the device ----
 // Sample resources (sample_resource.rs): one descriptor per uploaded resource; handles are index + 1.
@@ -44,41 +46,45 @@ struct SamplerMsgDev { uint32_t kind, a; uint64_t x, y; };  // SET_SAMPLE: a = h
 // (WRAP), or is zero (ZERO_TAIL, the sample ended), sampler.rs:445-516. CLEAR: clear_all_outputs.
 enum SmpMode : uint32_t { SMP_CLEAR = 0, SMP_PLAY = 1, SMP_PLAY_WRAP = 2, SMP_PLAY_ZERO_TAIL = 3 };
 struct SmpRec { uint64_t p0; uint32_t first, mode; };
-// polyphase resampler player (spec ours): what the control kernel needs for the silence flags (constant within a call)
-struct RsCtl { const uint32_t* flags; const uint32_t* res; const ResDesc* res_tab; uint32_t n_res, n_out; };  // flags: bit0 playing, bit1 loop
+// Every sampler and resampler of a context reads the same resource table; the control kernel gets this call's snapshot of it in
+// ControlArgs.
+struct RsCtl { const uint32_t* flags; const uint32_t* res; uint32_t n_out, pad; };  // flags: bit0 playing, bit1 loop
 struct SamplerCtl {
     // per-voice processor state (SamplerProcessor fields sampler.rs:283-297), persistent across calls
     uint32_t* playing; uint64_t* playhead; uint32_t* loop_flags;  // bit0: loop_range.is_some(), bit1: full_range
     uint64_t* loop_start; uint64_t* loop_end; uint32_t* res;      // res: resource handle, 0 = None
-    // per call
-    const ResDesc* res_tab; const SamplerMsgDev* msgs; const uint32_t* msg_off;  // messages of voice v: [msg_off[v], msg_off[v+1])
+    const SamplerMsgDev* msgs; const uint32_t* msg_off;           // the chunk's messages of voice v: [msg_off[v], msg_off[v+1])
     SmpRec* rec;                                                   // [block][voice]
-    uint32_t n_res, n_msgs, n_out, pad;
+    uint32_t* last_play;                                           // [voice]: the last block the walk processed played (scratch)
+    uint32_t n_out, pad;
 };
+// The schedule as the control kernel reads it: arrays of the plan, laid out one after the other (each 16-byte aligned) in one device
+// buffer, `image`, uploaded once when the graph is lowered; o_*: their byte offsets in it.
+//   nodes     CtlNode per scheduled node
+//   in_port   per input port: pool buffer | kPortClear when the port is unconnected (schedule.rs:310-313)
+//   out_port  per output port: pool buffer
+//   sm, smp, rs  SmDesc per smoother, SamplerCtl per SamplerNode, RsCtl per ResamplerNode
 struct CtlTables {
-    uint32_t n_nodes, n_smoothers, n_buffers, pad;
-    CtlNode nodes[kMaxCtlNodes];
-    uint8_t in_buf[kMaxCtlPorts], in_clear[kMaxCtlPorts], out_buf[kMaxCtlPorts];
-    // per-smoother state (SoA over voices, owned by the node's device state) and its target parameter
-    SamplerCtl smp[kMaxSamplers]; uint32_t n_samplers, n_resamplers;
-    RsCtl rs[kMaxSamplers];
-    float* sm_input[kMaxSmoothers];
-    float* sm_last[kMaxSmoothers];
-    uint32_t* sm_status[kMaxSmoothers];
-    const float* sm_target[kMaxSmoothers];
+    const void* image; uint32_t image_bytes, pad;
+    uint32_t o_nodes, o_in_port, o_out_port, o_sm, o_smp, o_rs;
+    uint32_t n_nodes, n_smoothers, n_buffers, n_flag_words;  // n_flag_words = ceil(n_buffers / 64)
+    uint32_t n_samplers, n_resamplers, n_in_ports, n_out_ports;
 };
+constexpr uint32_t kCtlParamImage = 2048;  // a table image up to this size also travels in the control kernel's parameters
+constexpr uint32_t kPortClear = 0x80000000u;
 
 // Per-call record buffers written by the control kernel, read by the data kernels.
-//   modes[k][v]          2 bits per smoother
+//   modes[k][w][v]       2 bits per smoother: smoother s in word w = s / 16, bits 2 (s % 16) (n_mode_words = max(1, ceil(NS / 16)))
 //   vals[k][s][v]        constant value of smoother s in block k (REC_CONST)
 //   curves[k][s][v][F]   gain curve (REC_CURVE)
 //   steady_k[v]          blocks >= steady_k[v] reuse the record of block steady_k[v]
-//   st_modes[v], st_vals[s][v]  that steady record, flattened so the data kernels reach it with one independent load
+//   st_modes[v]          OR of the steady record's mode words: 0 iff every smoother is REC_CONST there (the chain kernel's fast path)
+//   st_vals[s][v]        the steady record's constant values, flattened so the data kernels reach them with one independent load
 struct Records {
     uint32_t* modes; float* vals; float* curves; uint32_t* steady_k; uint64_t* gout_mask; uint32_t* error;
     uint32_t* st_modes; float* st_vals;
     uint64_t* sum_masks; uint64_t* st_sum_masks;  // [k][slot][v] and the steady record [slot][v]
-    uint32_t n_sum_masks, pad_;
+    uint32_t n_sum_masks, n_mode_words;
     uint32_t kt_max, n_smoothers;
     // Graphs with SamplerNodes: a sample that ends mid-call starts a new transient, so "record of block k" is no longer
     // min(k, steady_k): slot_of[k][v] names the record slot explicitly (null for graphs without samplers). steady_k[v] is
@@ -100,12 +106,18 @@ struct SamplerArgs {
 struct PokeArgs { void* ptr[16]; uint64_t val[16]; uint32_t count[16], stride_bytes[16]; uint8_t bytes[16]; uint32_t n; };
 
 struct ControlArgs {
-    CtlTables tables;      // by value: read through the constant bank (2.8 KB of kernel parameters)
+    CtlTables tables;
     Records rec;
-    uint64_t* flags;       // [V] buffer_silence_flags bitset (schedule.rs:170), persists across calls
+    uint64_t* flags;       // [n_flag_words][V] buffer_silence_flags bitset (schedule.rs:170), persists across calls
+    const ResDesc* smp_res_tab; const ResDesc* rs_res_tab;  // the resource table the samplers / resamplers read in this chunk
+    uint32_t smp_n_res, rs_n_res;
+    uint32_t smp_msgs;     // some sampler has messages in this chunk (else every msg_off is all zero)
+    uint32_t stage_tables; // set by launch_control: each CTA copies the table image to shared memory first
     uint32_t num_voices, frames, block_frames;
     float a, b, eps;       // smoother.rs:99-100,22
     uint32_t err_value;    // written to *rec.error on a record-budget overflow: (call epoch << 4) | 1
+    uint32_t image_in_param;  // `image` holds a copy of tables.image (small graphs: read with the launch, not from memory)
+    alignas(16) unsigned char image[kCtlParamImage];
 };
 
 struct ChainArgs {

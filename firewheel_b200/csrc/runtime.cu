@@ -162,6 +162,7 @@ struct NodeDeviceState {
     std::shared_ptr<ResTable> res_table;
     uint32_t* d_playing = nullptr; uint64_t* d_playhead = nullptr; uint32_t* d_loop_flags = nullptr; uint64_t* d_loop_start = nullptr; uint64_t* d_loop_end = nullptr; uint32_t* d_res = nullptr;
     SamplerMsgDev* d_msgs = nullptr; size_t cap_msgs = 0; uint32_t* d_msg_off = nullptr; uint32_t cur_n_msgs = 0;  // this chunk's messages on the device
+    bool msg_off_dirty = false;  // d_msg_off still holds the offsets of an earlier chunk's messages
     const ResDesc* cur_tab = nullptr; uint32_t cur_n_res = 0;
     // custom node (plugin vtable): the processor returned by activate() and the dense per-(block, voice) input masks handed to it
     void* custom_proc = nullptr; bool custom_deactivate = false;  // true: released through deactivate(node, processor) (graph.rs:603-609,644-648)
@@ -236,11 +237,16 @@ struct NodeDeviceState {
         d_msgs = mem.dev<SamplerMsgDev>(cap, false);
         return mem.ok() && FW_CUDA(cudaEventCreateWithFlags(&ev_staged, cudaEventDisableTiming));
     }
-    // cmds[0..n): the CMD_SAMPLER commands of this node for the chunk, in push order
-    bool stage_sampler(const Cmd* const* cmds, uint32_t n, cudaStream_t st) {
-        res_table->snapshot(&cur_tab, &cur_n_res);
+    // cmds[0..n): the CMD_SAMPLER commands of this node for the chunk, in push order; tab / n_res: the chunk's resource table. A chunk
+    // without messages leaves d_msg_off all zero: the control kernel reads the offsets of every sampler once any of them has messages.
+    bool stage_sampler(const Cmd* const* cmds, uint32_t n, const ResDesc* tab, uint32_t n_res, cudaStream_t st) {
+        cur_tab = tab; cur_n_res = n_res;
         cur_n_msgs = n;
-        if (n == 0) return true;
+        if (n == 0) {
+            if (!msg_off_dirty) return true;
+            msg_off_dirty = false;
+            return FW_CUDA(cudaMemsetAsync(d_msg_off, 0, ((size_t)V + 1) * sizeof(uint32_t), st));
+        }
         if (staged_pending) { cudaEventSynchronize(ev_staged); staged_pending = false; }  // the previous copy has read the pinned buffer (it precedes that chunk's kernels)
         std::memset(h_cnt, 0, ((size_t)V + 1) * sizeof(uint32_t));
         auto each_voice = [&](const Cmd& m, auto&& f) { if (m.voice == FW_ALL_VOICES) { for (uint32_t v = 0; v < V; ++v) f(v); } else if (m.voice < V) f(m.voice); };
@@ -254,12 +260,8 @@ struct NodeDeviceState {
         cur_n_msgs = (uint32_t)total;
         const bool ok = FW_CUDA(cudaMemcpyAsync(d_msgs, h_msgs, total * sizeof(SamplerMsgDev), cudaMemcpyHostToDevice, st)) &&
                         FW_CUDA(cudaMemcpyAsync(d_msg_off, h_off, ((size_t)V + 1) * sizeof(uint32_t), cudaMemcpyHostToDevice, st));
-        cudaEventRecord(ev_staged, st); staged_pending = true;
+        cudaEventRecord(ev_staged, st); staged_pending = true; msg_off_dirty = true;
         return ok;
-    }
-    // at call start: pin the resource table a resampler reads during this call
-    void snapshot_params() {
-        if (kind == FW_NODE_RESAMPLER) res_table->snapshot(&cur_tab, &cur_n_res);
     }
 };
 
@@ -268,6 +270,10 @@ struct Plan {
     Schedule sched;
     std::vector<std::shared_ptr<NodeDeviceState>> states;   // keeps every referenced node state alive
     std::vector<Id> nodes_to_remove;
+    // The control tables: built on the host by lower_control / lower_generic (smp[i].rec / last_play by alloc_plan), laid out as one
+    // image and uploaded once by alloc_plan; `tables` then describes the device image.
+    std::vector<CtlNode> nodes; std::vector<uint32_t> in_port, out_port; std::vector<SmDesc> sm; std::vector<SamplerCtl> smp; std::vector<RsCtl> rs;
+    std::vector<unsigned char> image;  // the tables laid out as CtlTables::image
     CtlTables tables{}; uint64_t* d_flags = nullptr;
     // Data plane: the steps run in order, each one launch group. An operand is C contiguous channels of one space: the caller's input or
     // output rows from channel `index` (row pitch Tfull, or n_in / n_out * Tfull for C == 1), pool buffer `index` of the generic lowering
@@ -376,8 +382,9 @@ struct fw_processor {
     uint32_t max_call_frames = 0; uint32_t call_epoch = 0, first_epoch_of_call = 0, synced_epoch = 0;
     std::vector<Cmd> pend; size_t pend_n = 0; std::vector<const Cmd*> cmd_ptrs;  // drained commands not yet applied (preallocated at activate)
     // CUDA-graph replay of steady chunks (SURVEY f2): the launch sequence of a chunk, captured once per (plan, buffers, frames)
+    // res_tab / n_res: the resource table every sampler of the plan reads (one snapshot per chunk, see apply_commands)
     struct GraphEntry { cudaGraphExec_t exec = nullptr; Plan* plan = nullptr; const float* d_in = nullptr; float* d_out = nullptr; uint32_t t0 = 0, Tc = 0, Tfull = 0;
-                        const void* tabs[2 * kMaxSamplers] = {}; uint32_t seen = 0; uint64_t stamp = 0; };
+                        const ResDesc* res_tab = nullptr; uint32_t n_res = 0; uint32_t seen = 0; uint64_t stamp = 0; };
     GraphEntry graphs[4]; uint64_t graph_stamp = 0, graph_replays = 0; bool capturing = false, graphs_off = false;
     // multi-GPU master bus: voices shard by rank; the per-rank buses are all-gathered and tree-summed in rank order
     void* nccl_comm = nullptr; int rank = 0, world = 1;
@@ -433,60 +440,79 @@ static bool chain_op(uint32_t kind, int sm0, float threshold_gain, ChainOp* op) 
 }
 
 // Control tables (one CtlNode per scheduled node, the smoothers, the sampler and resampler transport state) and the node states of
-// the plan. sm_of_node[i]: the first smoother of node i, -1: none.
+// the plan. sm_of_node[i]: the first smoother of node i, -1: none. Smoothers are numbered in schedule order (the control kernel
+// relies on it when it packs their modes).
 static bool lower_control(fw_ctx* c, const Schedule& s, Plan* plan, std::vector<int>* sm_of_node, std::string* why) {
     Graph& g = *c->graph;
     const size_t n = s.nodes.size();
-    if (n < 2 || n > (size_t)kMaxCtlNodes) { *why = "schedule too long for the device control tables"; return false; }
-    if (s.num_buffers > 64) { *why = "more than 64 buffers in one voice graph"; return false; }
+    if (n < 2) { *why = "schedule too short for the device control tables"; return false; }
     CtlTables& tb = plan->tables;
-    tb.n_nodes = (uint32_t)n; tb.n_buffers = s.num_buffers;
-    uint32_t off_in = 0, off_out = 0, n_sm = 0;
+    tb.n_nodes = (uint32_t)n; tb.n_buffers = s.num_buffers; tb.n_flag_words = std::max(1u, (s.num_buffers + 63u) / 64u);
+    if (control_threads(tb.n_flag_words, c->cfg.device) == 0) { *why = "the silence flags of one voice do not fit in the device's shared memory"; return false; }
+    uint32_t n_sm = 0;
     sm_of_node->assign(n, -1);
+    plan->nodes.assign(n, CtlNode{});
     for (size_t i = 0; i < n; ++i) {
         const SchedNode& sn = s.nodes[i];
         NodeRec* nr = g.node(sn.id);
-        CtlNode& cn = tb.nodes[i];
+        CtlNode& cn = plan->nodes[i];
         cn.kind = (uint8_t)nr->params->kind; cn.n_in = (uint8_t)sn.in.size(); cn.n_out = (uint8_t)sn.out.size();
-        cn.in_off = (uint16_t)off_in; cn.out_off = (uint16_t)off_out; cn.sm0 = cn.sm1 = -1;
-        if (nr->params->kind == FW_NODE_CUSTOM) cn.sm0 = (int16_t)nr->params->custom->info.out_silence_rule;
-        if (off_in + sn.in.size() > (size_t)kMaxCtlPorts || off_out + sn.out.size() > (size_t)kMaxCtlPorts) { *why = "too many ports"; return false; }
-        for (const InAssign& a : sn.in) { tb.in_buf[off_in] = (uint8_t)a.buffer; tb.in_clear[off_in] = a.should_clear; ++off_in; }
-        for (const OutAssign& a : sn.out) tb.out_buf[off_out++] = (uint8_t)a.buffer;
+        cn.in_off = (uint32_t)plan->in_port.size(); cn.out_off = (uint32_t)plan->out_port.size(); cn.sm0 = cn.sm1 = -1;
+        if (nr->params->kind == FW_NODE_CUSTOM) cn.sm0 = (int32_t)nr->params->custom->info.out_silence_rule;
+        for (const InAssign& a : sn.in) plan->in_port.push_back(a.buffer | (a.should_clear ? kPortClear : 0u));
+        for (const OutAssign& a : sn.out) plan->out_port.push_back(a.buffer);
         auto it = c->node_states.find(sn.id.pack());
         if (it == c->node_states.end()) { *why = "internal: node without device state"; return false; }
         std::shared_ptr<NodeDeviceState> st = it->second;
         plan->states.push_back(st);
         if (st->n_sm) {
-            if (n_sm + st->n_sm > (uint32_t)kMaxSmoothers) { *why = "more than 16 smoothed parameters in one voice graph"; return false; }
             (*sm_of_node)[i] = (int)n_sm;
-            cn.sm0 = (int16_t)n_sm; if (st->n_sm == 2) cn.sm1 = (int16_t)(n_sm + 1);
-            for (uint32_t k = 0; k < st->n_sm; ++k) {
-                tb.sm_input[n_sm] = st->sm_input[k]; tb.sm_last[n_sm] = st->sm_last[k]; tb.sm_status[n_sm] = st->sm_status[k]; tb.sm_target[n_sm] = st->d_target[k];
-                ++n_sm;
-            }
+            cn.sm0 = (int32_t)n_sm; if (st->n_sm == 2) cn.sm1 = (int32_t)(n_sm + 1);
+            for (uint32_t k = 0; k < st->n_sm; ++k, ++n_sm) plan->sm.push_back(SmDesc{st->sm_input[k], st->sm_last[k], st->sm_status[k], st->d_target[k]});
         }
     }
     tb.n_smoothers = n_sm; plan->n_sm = n_sm;
     for (size_t i = 0; i < n; ++i) {  // SamplerNodes: per-voice transport state lives in the node's device state
-        if (tb.nodes[i].kind != FW_NODE_SAMPLER) continue;
-        if (tb.n_samplers >= (uint32_t)kMaxSamplers) { *why = "more than 4 SamplerNodes in one voice graph"; return false; }
+        if (plan->nodes[i].kind != FW_NODE_SAMPLER) continue;
         const std::shared_ptr<NodeDeviceState>& st = plan->states[i];
-        SamplerCtl& sc = tb.smp[tb.n_samplers];
+        SamplerCtl sc{};
         sc.playing = st->d_playing; sc.playhead = st->d_playhead; sc.loop_flags = st->d_loop_flags; sc.loop_start = st->d_loop_start; sc.loop_end = st->d_loop_end; sc.res = st->d_res;
+        sc.msgs = st->d_msgs; sc.msg_off = st->d_msg_off;
         sc.n_out = (uint32_t)s.nodes[i].out.size();
-        tb.nodes[i].sm1 = (int16_t)tb.n_samplers++;
+        plan->nodes[i].sm1 = (int32_t)plan->smp.size();
+        plan->smp.push_back(sc);
         plan->samplers.push_back(st);
     }
     for (size_t i = 0; i < n; ++i) {
-        if (tb.nodes[i].kind != FW_NODE_RESAMPLER) continue;
-        if (tb.n_resamplers >= (uint32_t)kMaxSamplers) { *why = "more than 4 ResamplerNodes in one voice graph"; return false; }
+        if (plan->nodes[i].kind != FW_NODE_RESAMPLER) continue;
         const std::shared_ptr<NodeDeviceState>& st = plan->states[i];
-        RsCtl& rc = tb.rs[tb.n_resamplers];
-        rc.flags = st->d_rs_flags; rc.res = st->d_rs_res; rc.n_out = (uint32_t)s.nodes[i].out.size();
-        tb.nodes[i].sm1 = (int16_t)tb.n_resamplers++;
+        plan->nodes[i].sm1 = (int32_t)plan->rs.size();
+        plan->rs.push_back(RsCtl{st->d_rs_flags, st->d_rs_res, (uint32_t)s.nodes[i].out.size(), 0u});
         plan->resamplers.push_back(st);
     }
+    tb.n_samplers = (uint32_t)plan->smp.size(); tb.n_resamplers = (uint32_t)plan->rs.size();
+    tb.n_in_ports = (uint32_t)plan->in_port.size(); tb.n_out_ports = (uint32_t)plan->out_port.size();
+    return true;
+}
+
+// Appends `op` to a chain program and gives its smoothers program-local indices (ChainOp::l0 / l1, ChainProgram::sm). False, and the
+// program unchanged, when the program would read more than kMaxProgSmoothers distinct smoothers.
+static bool prog_push(ChainProgram& p, ChainOp op) {
+    uint32_t n_sm = p.n_sm;
+    int32_t sm[kMaxProgSmoothers];
+    std::copy(p.sm, p.sm + kMaxProgSmoothers, sm);
+    const int32_t g[2] = {op.sm0, op.sm1};
+    int32_t* l[2] = {&op.l0, &op.l1};
+    for (int k = 0; k < 2; ++k) {
+        *l[k] = -1;
+        if (g[k] < 0) continue;
+        uint32_t i = 0;
+        while (i < n_sm && sm[i] != g[k]) ++i;
+        if (i == n_sm) { if (n_sm == (uint32_t)kMaxProgSmoothers) return false; sm[n_sm++] = g[k]; }
+        *l[k] = (int32_t)i;
+    }
+    std::copy(sm, sm + kMaxProgSmoothers, p.sm); p.n_sm = n_sm;
+    p.ops[p.n_ops++] = op;
     return true;
 }
 
@@ -507,11 +533,11 @@ static bool lower_chain(const Schedule& s, const std::vector<int>& sm_of_node, b
     };
     Id prev = gin.id;
     size_t first = 1;
-    if (width == 0 && n >= 3 && plan->tables.nodes[1].kind == FW_NODE_SAMPLER && s.nodes[1].in.empty() && s.nodes[1].out.size() >= 1 && s.nodes[1].out.size() <= 2) {
+    if (width == 0 && n >= 3 && plan->nodes[1].kind == FW_NODE_SAMPLER && s.nodes[1].in.empty() && s.nodes[1].out.size() >= 1 && s.nodes[1].out.size() <= 2) {
         // no stream inputs: a SamplerNode heads the chain (BASELINE config 5: sampler -> gain -> pan -> ... -> bus)
         width = (uint32_t)s.nodes[1].out.size();
         stage(Plan::Step::SAMPLER, plan->states[1]);
-        steps.back().in.clear(); steps.back().sm0 = sm_of_node[1]; steps.back().sampler_idx = plan->tables.nodes[1].sm1;
+        steps.back().in.clear(); steps.back().sm0 = sm_of_node[1]; steps.back().sampler_idx = plan->nodes[1].sm1;
         prev = s.nodes[1].id; first = 2;
     }
     if (width < 1 || width > 2) { *why = "the fused chain supports 1 or 2 channels"; return false; }
@@ -552,7 +578,7 @@ static bool lower_chain(const Schedule& s, const std::vector<int>& sm_of_node, b
         }
         ChainOp op;
         if (!chain_op(kind, sm_of_node[i], np.threshold_gain, &op)) { *why = std::string("node kind '") + node_debug_name(kind) + "' has no device lowering yet"; return false; }
-        cur.ops[cur.n_ops++] = op;
+        if (!prog_push(cur, op)) { close_pointwise(false); prog_push(cur, op); }  // a program reads at most kMaxProgSmoothers smoothers
         width = (uint32_t)sn.out.size();
         prev = sn.id;
     }
@@ -594,8 +620,7 @@ static bool lower_generic(const Schedule& s, const std::vector<int>& sm_of_node,
              kind == FW_NODE_MONO_TO_STEREO || kind == FW_NODE_STEREO_TO_MONO)));
         if (kind == FW_NODE_CUSTOM && !np.custom->vt.process_device) { *why = std::string("custom node '") + np.custom->debug_name + "' has no process_device: it cannot run on the device (there is no CPU fallback)"; return false; }
         if (needs_mask) {
-            if (n_sum_masks >= (uint32_t)kMaxSumMasks) { *why = "more than 32 mask-dependent nodes in one voice graph"; return false; }
-            sp.mask_slot = (int)n_sum_masks; plan->tables.nodes[i].mask_slot = (uint8_t)(++n_sum_masks);
+            sp.mask_slot = (int)n_sum_masks; plan->nodes[i].mask_slot = ++n_sum_masks;
         }
         if (kind == FW_NODE_DUMMY && !endpoint && !sn.out.empty()) { *why = "a DummyAudioNode inside the graph leaves its outputs stale in the reference (dummy.rs:34-41): not reproducible on the device"; return false; }
         if (kind == FW_NODE_MONO_TO_STEREO && (sn.in.size() != 1 || sn.out.size() != 2)) { *why = "MonoToStereoNode must be 1 -> 2"; return false; }
@@ -609,7 +634,7 @@ static bool lower_generic(const Schedule& s, const std::vector<int>& sm_of_node,
             const bool bus_out = bus && i + 1 == n;
             sp.prog.c_in = sp.prog.c_out = bus_out ? (uint32_t)sn.in.size() : 2u; sp.pairs = !bus_out;
         } else if (chain_op(kind, sp.sm0, np.threshold_gain, &op)) {
-            sp.prog.n_ops = 1; sp.prog.ops[0] = op;
+            prog_push(sp.prog, op);
             sp.prog.c_in = kind == FW_NODE_MONO_TO_STEREO ? 1u : 2u; sp.prog.c_out = kind == FW_NODE_STEREO_TO_MONO ? 1u : 2u;
             sp.pairs = kind == FW_NODE_VOLUME || kind == FW_NODE_HARD_CLIP;
         } else if (kind == FW_NODE_BIQUAD || kind == FW_NODE_SVF || kind == FW_NODE_DELAY) {
@@ -618,7 +643,7 @@ static bool lower_generic(const Schedule& s, const std::vector<int>& sm_of_node,
         } else {
             sp.kind = kind == FW_NODE_SUM ? Plan::Step::SUM : kind == FW_NODE_SAMPLER ? Plan::Step::SAMPLER : kind == FW_NODE_CONV_REVERB ? Plan::Step::REVERB :
                       kind == FW_NODE_RESAMPLER ? Plan::Step::RESAMPLER : Plan::Step::CUSTOM;
-            if (kind == FW_NODE_SAMPLER) sp.sampler_idx = plan->tables.nodes[i].sm1;
+            if (kind == FW_NODE_SAMPLER) sp.sampler_idx = plan->nodes[i].sm1;
         }
         plan->steps.push_back(std::move(sp));
     }
@@ -689,7 +714,9 @@ static void fuse_generic(const Schedule& s, Plan* plan) {
         for (const Plan::Operand& o : st[i].out) for (const Plan::Operand& q : st[j].in) if (o.space == q.space && o.index == q.index) in_place = true;
         if (in_place) continue;
         ChainProgram pr = st[j].prog;
-        for (uint32_t k = 0; k < st[i].prog.n_ops; ++k) pr.ops[pr.n_ops++] = st[i].prog.ops[k];
+        bool fits = true;  // the run closes before its program would read more than kMaxProgSmoothers smoothers
+        for (uint32_t k = 0; k < st[i].prog.n_ops && fits; ++k) fits = prog_push(pr, st[i].prog.ops[k]);
+        if (!fits) continue;
         st[i].prog = pr; st[i].pairs = false;
         st[i].in = st[j].in;
         folded[j] = true;
@@ -704,9 +731,9 @@ static bool alloc_plan(const fw_ctx* c, Plan* plan, bool pool, std::string* why)
     const uint32_t V = c->cfg.num_voices, F = c->max_block_frames, n_sm = plan->n_sm;
     plan->num_voices = V; plan->block_frames = F; plan->bus = c->cfg.master_bus != 0;
     DevMem& mem = plan->mem;
-    plan->d_flags = mem.dev<uint64_t>(V);
+    plan->d_flags = mem.dev<uint64_t>((size_t)plan->tables.n_flag_words * V);
     Records& r = plan->rec;
-    r.n_smoothers = n_sm;
+    r.n_smoothers = n_sm; r.n_mode_words = std::max(1u, (n_sm + kModesPerWord - 1) / kModesPerWord);
     // Longest transient a record buffer must hold: a ramp decays like b^n with tau = smooth_secs * sample_rate samples and settles at
     // |delta| * b^n < 1e-5 (smoother.rs:99-100,179); sized for |delta| up to 1e4 (a jump of 10000 % in percent_volume): ln(1e9) tau.
     // A chunk never has more blocks than chunk_blocks, so min() with that is enough when the chunk is shorter than the ramp.
@@ -717,7 +744,7 @@ static bool alloc_plan(const fw_ctx* c, Plan* plan, bool pool, std::string* why)
         r.kt_max = (n_sm ? ramp_blocks : 4u) + 8u * (uint32_t)plan->samplers.size();  // every sample that ends mid-call opens a short transient of its own
         r.kt_max = std::max(2u, std::min(r.kt_max, kc));
     }
-    r.modes = mem.dev<uint32_t>((size_t)r.kt_max * V);
+    r.modes = mem.dev<uint32_t>((size_t)r.kt_max * r.n_mode_words * V);
     r.vals = mem.dev<float>((size_t)r.kt_max * (n_sm ? n_sm : 1) * V);
     r.curves = mem.dev<float>((size_t)r.kt_max * n_sm * V * F, false);
     r.steady_k = mem.dev<uint32_t>(V);
@@ -741,10 +768,28 @@ static bool alloc_plan(const fw_ctx* c, Plan* plan, bool pool, std::string* why)
         if (pool) plan->d_pool = mem.dev<float>((size_t)plan->num_buffers * V * Tc, false);
         if (!plan->samplers.empty()) {
             plan->d_slot_of = mem.dev<uint16_t>((size_t)Kc * V);
-            for (size_t i = 0; i < plan->samplers.size(); ++i) plan->d_srec.push_back(mem.dev<SmpRec>((size_t)Kc * V));
+            for (size_t i = 0; i < plan->samplers.size(); ++i) {
+                plan->d_srec.push_back(mem.dev<SmpRec>((size_t)Kc * V));
+                plan->smp[i].rec = plan->d_srec.back(); plan->smp[i].last_play = mem.dev<uint32_t>(V);
+            }
         }
         for (auto& sp : plan->steps) if (sp.kind == Plan::Step::CUSTOM) { sp.custom_idx = (int)plan->d_custom_masks.size(); plan->d_custom_masks.push_back(mem.dev<uint64_t>((size_t)Kc * V)); }
         r.slot_of = plan->d_slot_of;
+    }
+    {   // the control tables as one image (CtlTables), uploaded once
+        CtlTables& tb = plan->tables;
+        std::vector<unsigned char>& im = plan->image;
+        auto put = [&](const auto& h) {
+            const size_t o = im.size(), n = h.size() * sizeof(h[0]);
+            im.resize(o + ((n + 15) & ~(size_t)15));
+            if (n) std::memcpy(im.data() + o, h.data(), n);
+            return o;
+        };
+        const size_t o_nodes = put(plan->nodes), o_in = put(plan->in_port), o_out = put(plan->out_port), o_sm = put(plan->sm), o_smp = put(plan->smp), o_rs = put(plan->rs);
+        unsigned char* d = mem.dev<unsigned char>(im.size(), false);
+        if (!d || (!im.empty() && !FW_CUDA(cudaMemcpy(d, im.data(), im.size(), cudaMemcpyHostToDevice)))) { *why = "control table upload failed: " + g_dev_err; return false; }
+        tb.image = d; tb.image_bytes = (uint32_t)im.size();
+        tb.o_nodes = (uint32_t)o_nodes; tb.o_in_port = (uint32_t)o_in; tb.o_out_port = (uint32_t)o_out; tb.o_sm = (uint32_t)o_sm; tb.o_smp = (uint32_t)o_smp; tb.o_rs = (uint32_t)o_rs;
     }
     if (!mem.ok()) { *why = "device allocation failed: " + g_dev_err; return false; }
     return true;
@@ -1646,10 +1691,12 @@ static bool apply_commands(fw_processor* p, Plan& pl, uint32_t b) {
     }
     pk.flush();
     if (!pk.ok) return false;
+    const ResDesc* tab = nullptr; uint32_t n_res = 0;  // one snapshot for every sampler of the chunk (they share the context's table)
+    if (!pl.samplers.empty()) pl.samplers[0]->res_table->snapshot(&tab, &n_res);
     for (auto& st : pl.samplers) {
         uint32_t n = 0;
         for (size_t i = 0; i < p->pend_n; ++i) { const Cmd& m = p->pend[i]; if (m.block == b && m.kind == CMD_SAMPLER && m.node == st->params.get()) p->cmd_ptrs[n++] = &m; }
-        if (!st->stage_sampler(p->cmd_ptrs.data(), n, p->stream)) return false;
+        if (!st->stage_sampler(p->cmd_ptrs.data(), n, tab, n_res, p->stream)) return false;
     }
     return true;
 }
@@ -1661,12 +1708,10 @@ static int enqueue_chunk(fw_processor* p, Plan& pl, const float* d_in, float* d_
     ++p->call_epoch;
     ControlArgs ca{};
     ca.tables = pl.tables; ca.rec = pl.rec;
-    for (size_t i = 0; i < pl.resamplers.size(); ++i) { ca.tables.rs[i].res_tab = pl.resamplers[i]->cur_tab; ca.tables.rs[i].n_res = pl.resamplers[i]->cur_n_res; }
-    for (size_t i = 0; i < pl.samplers.size(); ++i) {
-        NodeDeviceState& st = *pl.samplers[i];
-        SamplerCtl& sc = ca.tables.smp[i];
-        sc.res_tab = st.cur_tab; sc.n_res = st.cur_n_res; sc.msgs = st.d_msgs; sc.msg_off = st.d_msg_off; sc.n_msgs = st.cur_n_msgs; sc.rec = pl.d_srec[i];
-    }
+    if (!pl.resamplers.empty()) { ca.rs_res_tab = pl.resamplers[0]->cur_tab; ca.rs_n_res = pl.resamplers[0]->cur_n_res; }
+    if (!pl.samplers.empty()) { ca.smp_res_tab = pl.samplers[0]->cur_tab; ca.smp_n_res = pl.samplers[0]->cur_n_res; }
+    for (auto& st : pl.samplers) if (st->cur_n_msgs) ca.smp_msgs = 1;
+    if (pl.image.size() <= sizeof(ca.image)) { std::memcpy(ca.image, pl.image.data(), pl.image.size()); ca.image_in_param = 1; }
     ca.flags = pl.d_flags; ca.num_voices = V; ca.frames = T; ca.block_frames = pl.block_frames;
     ca.a = p->sm_a; ca.b = p->sm_b; ca.eps = p->sm_eps; ca.err_value = ((p->capturing ? kGraphEpoch : p->call_epoch) << 4) | 1u;
     if (!FW_LAUNCH(p, 0, 1, launch_control(ca, p->stream))) return FW_PROC_DEVICE_ERROR;
@@ -1774,17 +1819,17 @@ static int enqueue_chunk(fw_processor* p, Plan& pl, const float* d_in, float* d_
 // kernels' run time). Programmatic-dependent-launch edges are kept by the capture.
 static int run_chunk(fw_processor* p, Plan& pl, const float* d_in, float* d_out, const Chunk& ck, bool steady) {
     if (!steady || !pl.graphable || p->graphs_off || p->profiling || p->world > 1 || ck.zero_first) return enqueue_chunk(p, pl, d_in, d_out, ck);
-    const void* tabs[2 * kMaxSamplers] = {};
-    for (size_t i = 0; i < pl.samplers.size() && i < (size_t)kMaxSamplers; ++i) { tabs[2 * i] = pl.samplers[i]->cur_tab; tabs[2 * i + 1] = reinterpret_cast<const void*>((uintptr_t)pl.samplers[i]->cur_n_res); }
+    const ResDesc* res_tab = pl.samplers.empty() ? nullptr : pl.samplers[0]->cur_tab;
+    const uint32_t n_res = pl.samplers.empty() ? 0u : pl.samplers[0]->cur_n_res;
     fw_processor::GraphEntry* e = nullptr; fw_processor::GraphEntry* lru = &p->graphs[0];
     for (auto& g : p->graphs) {
-        if (g.plan == &pl && g.d_in == d_in && g.d_out == d_out && g.t0 == ck.t0 && g.Tc == ck.Tc && g.Tfull == ck.Tfull && std::memcmp(g.tabs, tabs, sizeof(tabs)) == 0) { e = &g; break; }
+        if (g.plan == &pl && g.d_in == d_in && g.d_out == d_out && g.t0 == ck.t0 && g.Tc == ck.Tc && g.Tfull == ck.Tfull && g.res_tab == res_tab && g.n_res == n_res) { e = &g; break; }
         if (g.stamp < lru->stamp) lru = &g;
     }
     if (!e) {  // first sight: remember the key, run normally
         e = lru;
         if (e->exec) { cudaGraphExecDestroy(e->exec); e->exec = nullptr; }
-        e->plan = &pl; e->d_in = d_in; e->d_out = d_out; e->t0 = ck.t0; e->Tc = ck.Tc; e->Tfull = ck.Tfull; std::memcpy(e->tabs, tabs, sizeof(tabs)); e->seen = 0;
+        e->plan = &pl; e->d_in = d_in; e->d_out = d_out; e->t0 = ck.t0; e->Tc = ck.Tc; e->Tfull = ck.Tfull; e->res_tab = res_tab; e->n_res = n_res; e->seen = 0;
     }
     e->stamp = ++p->graph_stamp;
     if (e->exec) {
@@ -1859,7 +1904,11 @@ static int proc_call(fw_processor* p, const float* d_in, float* d_out, uint32_t 
         if (!p->running) { silence_from(b * F); rc = FW_PROC_DROP_PROCESSOR; break; }        // :150-155
         Plan& pl = *p->plan;
         if (n_in != pl.c_in || n_out != pl.c_out) { g_dev_err = "channel counts do not match the compiled graph"; return FW_PROC_BAD_ARGS; }
-        if (b == 0) for (auto& st : pl.states) st->snapshot_params();
+        if (b == 0 && !pl.resamplers.empty()) {  // pin the resource table the resamplers read during this call
+            const ResDesc* tab; uint32_t n_res;
+            pl.resamplers[0]->res_table->snapshot(&tab, &n_res);
+            for (auto& st : pl.resamplers) { st->cur_tab = tab; st->cur_n_res = n_res; }
+        }
         while (next_cmd < p->pend_n && p->pend[next_cmd].block < b) ++next_cmd;
         const bool have_cmds = next_cmd < p->pend_n && p->pend[next_cmd].block == b;
         if (have_cmds || !pl.samplers.empty()) { if (!apply_commands(p, pl, b)) return FW_PROC_DEVICE_ERROR; }

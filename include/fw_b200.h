@@ -197,7 +197,11 @@ enum fw_compile_error {
     FW_COMPILE_MANY_TO_ONE = 5,
     FW_COMPILE_NODE_ACTIVATION_FAILED = 6,
     FW_COMPILE_MESSAGE_CHANNEL_FULL = 7,
-    /* product only: the graph is valid for the reference but has no device lowering yet */
+    /* product only: the graph is valid for the reference but has no device lowering yet. The refusals: a user node without
+     * process_device; a DummyAudioNode with outputs inside the graph; a MonoToStereoNode that is not 1 -> 2 or a StereoToMonoNode that
+     * is not 2 -> 1; a master bus over more than FW_MAX_BUS_CHANNELS graph_out channels; stream channel counts other than graph_in's /
+     * graph_out's port counts; silence flags of one voice that do not fit in one SM's shared memory (about 930 000 pool buffers on an
+     * H100). The number of nodes, buffers, ports, smoothed parameters, samplers and resamplers is not limited otherwise. */
     FW_COMPILE_UNSUPPORTED_ON_DEVICE = 100
 };
 /* FirewheelProcessorStatus (processor.rs:12-16) + device-error code */
