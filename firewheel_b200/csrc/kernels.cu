@@ -178,7 +178,7 @@ __global__ void __launch_bounds__(128) control_kernel(const __grid_constant__ Co
         for (uint32_t s = 0; s < NSMP; ++s) {
             const SamplerCtl& sc = smp[s];
             SmpLocal q = smp_load(sc, v);
-            smp_apply_messages(q, sc, v, a.smp_res_tab, a.smp_n_res);
+            smp_apply_messages(q, sc, v, a.res_tab, a.n_res);
             smp_store(sc, v, q);
         }
     }
@@ -198,7 +198,7 @@ __global__ void __launch_bounds__(128) control_kernel(const __grid_constant__ Co
                 const SamplerCtl& sc = smp[s];
                 if (!sc.last_play[v]) continue;
                 const uint32_t res = sc.res[v];
-                if (!(sc.loop_flags[v] & 1u) && sc.playhead[v] + frames > a.smp_res_tab[res - 1].frames) evt = true;
+                if (!(sc.loop_flags[v] & 1u) && sc.playhead[v] + frames > a.res_tab[res - 1].frames) evt = true;
             }
             if (!evt) {
                 for (uint32_t s = 0; s < NSMP; ++s) {
@@ -207,7 +207,7 @@ __global__ void __launch_bounds__(128) control_kernel(const __grid_constant__ Co
                     if (sc.last_play[v]) {
                         SmpLocal q = smp_load(sc, v);
                         bool dummy = false;
-                        smp_step(q, a.smp_res_tab[q.res - 1].frames, frames, &r, dummy);
+                        smp_step(q, a.res_tab[q.res - 1].frames, frames, &r, dummy);
                         sc.playhead[v] = q.playhead;  // the only field a replayed block moves
                     }
                     sc.rec[(size_t)k * V + v] = r;
@@ -303,8 +303,8 @@ __global__ void __launch_bounds__(128) control_kernel(const __grid_constant__ Co
                     SmpLocal q = smp_load(sc, v);
                     SmpRec r; r.p0 = 0; r.first = 0; r.mode = SMP_CLEAR;
                     bool play = false; uint32_t sch = 0;
-                    if (q.res != 0 && q.res <= a.smp_n_res && q.playing) {
-                        const ResDesc rd = a.smp_res_tab[q.res - 1];
+                    if (q.res != 0 && q.res <= a.n_res && q.playing) {
+                        const ResDesc rd = a.res_tab[q.res - 1];
                         sch = rd.channels;
                         const SmDesc d = smd[nd.sm0];
                         SmLocal s = sm_load(d, v);
@@ -329,8 +329,8 @@ __global__ void __launch_bounds__(128) control_kernel(const __grid_constant__ Co
                 case FW_NODE_RESAMPLER: {  // spec ours: cleared + flagged when not playing / no resource; surplus channels as the sampler's
                     const RsCtl rc = rsc[nd.sm1];
                     const uint32_t r = rc.res[v];
-                    if (!(rc.flags[v] & 1u) || r == 0 || r > a.rs_n_res) out_mask = all_silent_mask(nd.n_out);
-                    else { const uint32_t sch = a.rs_res_tab[r - 1].channels; if (nd.n_out > sch && !(nd.n_out == 2 && sch == 1)) out_mask = all_silent_mask(nd.n_out) & ~all_silent_mask(sch); }
+                    if (!(rc.flags[v] & 1u) || r == 0 || r > a.n_res) out_mask = all_silent_mask(nd.n_out);
+                    else { const uint32_t sch = a.res_tab[r - 1].channels; if (nd.n_out > sch && !(nd.n_out == 2 && sch == 1)) out_mask = all_silent_mask(nd.n_out) & ~all_silent_mask(sch); }
                     break;
                 }
                 case FW_NODE_SUM:  // sum.rs:52-65; the unrolled / generic sums never write the mask (Q7)

@@ -46,8 +46,8 @@ struct SamplerMsgDev { uint32_t kind, a; uint64_t x, y; };  // SET_SAMPLE: a = h
 // (WRAP), or is zero (ZERO_TAIL, the sample ended), sampler.rs:445-516. CLEAR: clear_all_outputs.
 enum SmpMode : uint32_t { SMP_CLEAR = 0, SMP_PLAY = 1, SMP_PLAY_WRAP = 2, SMP_PLAY_ZERO_TAIL = 3 };
 struct SmpRec { uint64_t p0; uint32_t first, mode; };
-// Every sampler and resampler of a context reads the same resource table; the control kernel gets this call's snapshot of it in
-// ControlArgs.
+// Every sampler and resampler of a context reads the same resource table; each chunk takes one snapshot of it (table and count), which
+// the control, sampler and resampler kernels of the chunk all read.
 struct RsCtl { const uint32_t* flags; const uint32_t* res; uint32_t n_out, pad; };  // flags: bit0 playing, bit1 loop
 struct SamplerCtl {
     // per-voice processor state (SamplerProcessor fields sampler.rs:283-297), persistent across calls
@@ -109,8 +109,7 @@ struct ControlArgs {
     CtlTables tables;
     Records rec;
     uint64_t* flags;       // [n_flag_words][V] buffer_silence_flags bitset (schedule.rs:170), persists across calls
-    const ResDesc* smp_res_tab; const ResDesc* rs_res_tab;  // the resource table the samplers / resamplers read in this chunk
-    uint32_t smp_n_res, rs_n_res;
+    const ResDesc* res_tab; uint32_t n_res;  // the chunk's snapshot of the resource table
     uint32_t smp_msgs;     // some sampler has messages in this chunk (else every msg_off is all zero)
     uint32_t stage_tables; // set by launch_control: each CTA copies the table image to shared memory first
     uint32_t num_voices, frames, block_frames;

@@ -80,23 +80,7 @@ class DevMem {
     std::vector<void*> dev_, host_; bool ok_ = true;
 };
 
-// wait-free SPSC ring (rtrb::RingBuffer, context.rs:61-64), capacity 16
-template <class T, size_t N = 16> struct Spsc {
-    T slots[N + 1];
-    std::atomic<size_t> head{0}, tail{0};
-    bool push(const T& v) {
-        size_t t = tail.load(std::memory_order_relaxed), n = (t + 1) % (N + 1);
-        if (n == head.load(std::memory_order_acquire)) return false;
-        slots[t] = v; tail.store(n, std::memory_order_release); return true;
-    }
-    bool pop(T* out) {
-        size_t h = head.load(std::memory_order_relaxed);
-        if (h == tail.load(std::memory_order_acquire)) return false;
-        *out = slots[h]; head.store((h + 1) % (N + 1), std::memory_order_release); return true;
-    }
-};
-
-// same, capacity chosen at run time (the command ring: sized from the voice count at activate)
+// wait-free SPSC ring (rtrb::RingBuffer, context.rs:61-64) of a capacity chosen at construction
 template <class T> struct DynSpsc {
     std::unique_ptr<T[]> slots; size_t n = 0;  // n = capacity + 1
     std::atomic<size_t> head{0}, tail{0};
@@ -158,12 +142,10 @@ struct NodeDeviceState {
     // polyphase resampler: table + per-voice transport mirrors + the device-resident Q32.32 position
     float* d_rs_table = nullptr; uint32_t* d_rs_res = nullptr; uint32_t* d_rs_flags = nullptr; uint64_t* d_rs_step = nullptr;
     uint64_t* d_rs_pos = nullptr;
-    // sampler: per-voice SamplerProcessor state (sampler.rs:283-297) + this call's messages / resource table / block records
-    std::shared_ptr<ResTable> res_table;
+    // sampler: per-voice SamplerProcessor state (sampler.rs:283-297) + this chunk's messages
     uint32_t* d_playing = nullptr; uint64_t* d_playhead = nullptr; uint32_t* d_loop_flags = nullptr; uint64_t* d_loop_start = nullptr; uint64_t* d_loop_end = nullptr; uint32_t* d_res = nullptr;
     SamplerMsgDev* d_msgs = nullptr; size_t cap_msgs = 0; uint32_t* d_msg_off = nullptr; uint32_t cur_n_msgs = 0;  // this chunk's messages on the device
     bool msg_off_dirty = false;  // d_msg_off still holds the offsets of an earlier chunk's messages
-    const ResDesc* cur_tab = nullptr; uint32_t cur_n_res = 0;
     // custom node (plugin vtable): the processor returned by activate() and the dense per-(block, voice) input masks handed to it
     void* custom_proc = nullptr; bool custom_deactivate = false;  // true: released through deactivate(node, processor) (graph.rs:603-609,644-648)
     explicit NodeDeviceState(int device) : mem(device) {}
@@ -237,10 +219,9 @@ struct NodeDeviceState {
         d_msgs = mem.dev<SamplerMsgDev>(cap, false);
         return mem.ok() && FW_CUDA(cudaEventCreateWithFlags(&ev_staged, cudaEventDisableTiming));
     }
-    // cmds[0..n): the CMD_SAMPLER commands of this node for the chunk, in push order; tab / n_res: the chunk's resource table. A chunk
-    // without messages leaves d_msg_off all zero: the control kernel reads the offsets of every sampler once any of them has messages.
-    bool stage_sampler(const Cmd* const* cmds, uint32_t n, const ResDesc* tab, uint32_t n_res, cudaStream_t st) {
-        cur_tab = tab; cur_n_res = n_res;
+    // cmds[0..n): the CMD_SAMPLER commands of this node for the chunk, in push order. A chunk without messages leaves d_msg_off all
+    // zero: the control kernel reads the offsets of every sampler once any of them has messages.
+    bool stage_sampler(const Cmd* const* cmds, uint32_t n, cudaStream_t st) {
         cur_n_msgs = n;
         if (n == 0) {
             if (!msg_off_dirty) return true;
@@ -296,7 +277,7 @@ struct Plan {
     uint32_t num_buffers = 0;  // generic lowering: pool buffers
     bool reads_caller_rows = false;  // some node reads the caller's input rows directly (row pitch n_in * frames must fit 32 bits)
     std::vector<std::shared_ptr<NodeDeviceState>> samplers;  // index = CtlTables::smp index
-    std::vector<std::shared_ptr<NodeDeviceState>> resamplers;  // index = CtlTables::rs index
+    std::shared_ptr<ResTable> res;  // the context's sample resources, which every sampler and resampler reads (null: the plan has neither)
     bool bus = false; uint32_t n_sm = 0, c_in = 0, c_out = 0, num_voices = 0, block_frames = 0;
     Records rec{};
     uint64_t* d_bus_mask = nullptr;
@@ -309,7 +290,6 @@ struct Plan {
     float* d_tmp[2] = {nullptr, nullptr};      // inter-stage scratch [V][2][chunk]
     float* d_pool = nullptr;                   // generic lowering: [buffer][V][chunk]
     uint16_t* d_slot_of = nullptr;             // sampler graphs: record slot per (block, voice)
-    std::vector<SmpRec*> d_srec;               // per SamplerNode: [block][voice]
     std::vector<uint64_t*> d_custom_masks;     // per custom node (index = Step::custom_idx): dense [block][voice] input masks
     DevMem mem;  // d_flags, the records, d_bus_mask and the scratch; declared last so that it frees them before the node states go
 };
@@ -343,11 +323,11 @@ static NcclApi g_nccl;
 struct CtxToProc { int kind = 0; Plan* plan = nullptr; };                 // 0 NewSchedule, 1 Stop (processor.rs:265-268)
 struct ProcToCtx { int kind = 0; Plan* plan = nullptr; void* user_cx = nullptr; };  // 0 ReturnSchedule, 1 Dropped (:270-277)
 struct Channels {
-    Spsc<CtxToProc> to_proc; Spsc<ProcToCtx> to_ctx;
-    DynSpsc<Cmd> cmds;                        // sampler messages, timed parameter stores, resampler transport (see Cmd)
+    DynSpsc<CtxToProc> to_proc; DynSpsc<ProcToCtx> to_ctx;  // capacity 16 (context.rs:61-64)
+    DynSpsc<Cmd> cmds;                        // sampler messages, timed parameter stores, resampler transport (see Cmd); sized from the voice count at activate
     DynSpsc<float*> to_free;                  // CMD_UPLOAD snapshots on their way back to the main thread, which frees them
     std::atomic<uint32_t> drain_epoch{1};     // bumped by the stream side after it emptied `cmds` (per-voice ring-full accounting)
-    explicit Channels(size_t cmd_capacity) : cmds(cmd_capacity), to_free(cmd_capacity) {}
+    explicit Channels(size_t cmd_capacity) : to_proc(16), to_ctx(16), cmds(cmd_capacity), to_free(cmd_capacity) {}
     ~Channels() { float* q; while (to_free.pop(&q)) delete[] q; Cmd m; while (cmds.pop(&m)) if (m.kind == CMD_UPLOAD) delete[] reinterpret_cast<float*>(m.x); }
 };
 
@@ -379,10 +359,10 @@ struct fw_processor {
     double cur_stream_time = 0.0; uint32_t cur_stream_status = 0;  // ProcInfo fields of the call being enqueued (node.rs:108-114)
     // I/O staging of the host-buffer entry points, allocated at activate for max_call_frames (the stream side never allocates)
     float *d_in = nullptr, *d_out = nullptr, *d_inter = nullptr, *d_flush = nullptr;
-    uint32_t max_call_frames = 0; uint32_t call_epoch = 0, first_epoch_of_call = 0, synced_epoch = 0;
+    uint32_t max_call_frames = 0; uint32_t call_epoch = 0, synced_epoch = 0;
     std::vector<Cmd> pend; size_t pend_n = 0; std::vector<const Cmd*> cmd_ptrs;  // drained commands not yet applied (preallocated at activate)
     // CUDA-graph replay of steady chunks (SURVEY f2): the launch sequence of a chunk, captured once per (plan, buffers, frames)
-    // res_tab / n_res: the resource table every sampler of the plan reads (one snapshot per chunk, see apply_commands)
+    // res_tab / n_res: the chunk's snapshot of the resource table (see Chunk)
     struct GraphEntry { cudaGraphExec_t exec = nullptr; Plan* plan = nullptr; const float* d_in = nullptr; float* d_out = nullptr; uint32_t t0 = 0, Tc = 0, Tfull = 0;
                         const ResDesc* res_tab = nullptr; uint32_t n_res = 0; uint32_t seen = 0; uint64_t stamp = 0; };
     GraphEntry graphs[4]; uint64_t graph_stamp = 0, graph_replays = 0; bool capturing = false, graphs_off = false;
@@ -488,9 +468,9 @@ static bool lower_control(fw_ctx* c, const Schedule& s, Plan* plan, std::vector<
         const std::shared_ptr<NodeDeviceState>& st = plan->states[i];
         plan->nodes[i].sm1 = (int32_t)plan->rs.size();
         plan->rs.push_back(RsCtl{st->d_rs_flags, st->d_rs_res, (uint32_t)s.nodes[i].out.size(), 0u});
-        plan->resamplers.push_back(st);
     }
     tb.n_samplers = (uint32_t)plan->smp.size(); tb.n_resamplers = (uint32_t)plan->rs.size();
+    if (tb.n_samplers || tb.n_resamplers) plan->res = c->res;
     tb.n_in_ports = (uint32_t)plan->in_port.size(); tb.n_out_ports = (uint32_t)plan->out_port.size();
     return true;
 }
@@ -769,8 +749,7 @@ static bool alloc_plan(const fw_ctx* c, Plan* plan, bool pool, std::string* why)
         if (!plan->samplers.empty()) {
             plan->d_slot_of = mem.dev<uint16_t>((size_t)Kc * V);
             for (size_t i = 0; i < plan->samplers.size(); ++i) {
-                plan->d_srec.push_back(mem.dev<SmpRec>((size_t)Kc * V));
-                plan->smp[i].rec = plan->d_srec.back(); plan->smp[i].last_play = mem.dev<uint32_t>(V);
+                plan->smp[i].rec = mem.dev<SmpRec>((size_t)Kc * V); plan->smp[i].last_play = mem.dev<uint32_t>(V);
             }
         }
         for (auto& sp : plan->steps) if (sp.kind == Plan::Step::CUSTOM) { sp.custom_idx = (int)plan->d_custom_masks.size(); plan->d_custom_masks.push_back(mem.dev<uint64_t>((size_t)Kc * V)); }
@@ -1414,7 +1393,7 @@ int fw_ctx_update(fw_ctx* c, fw_update_status* out) {  // context.rs:93-148
                     ds->custom_proc = proc_h;
                 }
             }
-            if (ds->kind == FW_NODE_SAMPLER || ds->kind == FW_NODE_RESAMPLER) { if (!c->res) c->res = std::make_shared<ResTable>(c->cfg.device); ds->res_table = c->res; }
+            if ((ds->kind == FW_NODE_SAMPLER || ds->kind == FW_NODE_RESAMPLER) && !c->res) c->res = std::make_shared<ResTable>(c->cfg.device);
             if (!ds->create()) msg = "device allocation failed: " + g_dev_err;
         }
         if (!msg.empty()) {
@@ -1490,8 +1469,9 @@ static void proc_poll(fw_processor* p) {  // processor.rs:167-206
         for (auto& g : p->graphs) { if (g.exec) cudaGraphExecDestroy(g.exec); g = fw_processor::GraphEntry{}; }  // captured sequences point into the old plan
     }
 }
-// One chunk of a call: frames [t0, t0 + Tc) of rows that are Tfull frames long in the caller's buffers.
-struct Chunk { uint32_t t0, Tc, Tfull, zero_first; };
+// One chunk of a call: frames [t0, t0 + Tc) of rows that are Tfull frames long in the caller's buffers. res_tab / n_res: the snapshot of
+// the plan's resource table that every sampler and resampler reads in this chunk (see proc_call).
+struct Chunk { uint32_t t0, Tc, Tfull, zero_first; const ResDesc* res_tab; uint32_t n_res; };
 
 // One chain-kernel launch of `prog` over the chunk: channel c of voice v is read at in[c] + v * in_vs and written at out[c] + v * out_vs
 // (floats); an unused second channel repeats channel 0, and the bus stage reads all `prog.c_in` (up to kMaxBusChannels). `caller`: `in`
@@ -1576,14 +1556,14 @@ struct RowBlock { const float* in; float* out; uint32_t C; uint64_t in_pitch, ou
 static uint32_t channels_of(const RowBlock* b, uint32_t nb) { uint32_t n = 0; for (uint32_t i = 0; i < nb; ++i) n += b[i].C; return n; }
 
 // SamplerNode: one launch writes the output rows of every block.
-static int run_sampler(fw_processor* p, const Plan& pl, const NodeDeviceState& st, const SmpRec* srec, int sm, const RowBlock* b, uint32_t nb, uint32_t T) {
+static int run_sampler(fw_processor* p, const Plan& pl, const Chunk& ck, const NodeDeviceState& st, const SmpRec* srec, int sm, const RowBlock* b, uint32_t nb) {
     SamplerArgs sa{};
     for (uint32_t i = 0; i < nb; ++i) {
         for (uint32_t k = 0; k < b[i].C; ++k) sa.out[sa.n_out++] = b[i].out + k * b[i].out_pitch;
         sa.out_vstride = b[i].C * b[i].out_pitch;
     }
-    sa.num_voices = p->num_voices; sa.frames = T; sa.block_frames = pl.block_frames;
-    sa.srec = srec; sa.res = st.d_res; sa.loop_start = st.d_loop_start; sa.res_tab = st.cur_tab; sa.sm = sm; sa.rec = pl.rec;
+    sa.num_voices = p->num_voices; sa.frames = ck.Tc; sa.block_frames = pl.block_frames;
+    sa.srec = srec; sa.res = st.d_res; sa.loop_start = st.d_loop_start; sa.res_tab = ck.res_tab; sa.sm = sm; sa.rec = pl.rec;
     return FW_LAUNCH(p, 1, 1, launch_sampler(sa, p->stream)) ? FW_PROC_OK : FW_PROC_DEVICE_ERROR;
 }
 
@@ -1691,12 +1671,10 @@ static bool apply_commands(fw_processor* p, Plan& pl, uint32_t b) {
     }
     pk.flush();
     if (!pk.ok) return false;
-    const ResDesc* tab = nullptr; uint32_t n_res = 0;  // one snapshot for every sampler of the chunk (they share the context's table)
-    if (!pl.samplers.empty()) pl.samplers[0]->res_table->snapshot(&tab, &n_res);
     for (auto& st : pl.samplers) {
         uint32_t n = 0;
         for (size_t i = 0; i < p->pend_n; ++i) { const Cmd& m = p->pend[i]; if (m.block == b && m.kind == CMD_SAMPLER && m.node == st->params.get()) p->cmd_ptrs[n++] = &m; }
-        if (!st->stage_sampler(p->cmd_ptrs.data(), n, tab, n_res, p->stream)) return false;
+        if (!st->stage_sampler(p->cmd_ptrs.data(), n, p->stream)) return false;
     }
     return true;
 }
@@ -1708,8 +1686,7 @@ static int enqueue_chunk(fw_processor* p, Plan& pl, const float* d_in, float* d_
     ++p->call_epoch;
     ControlArgs ca{};
     ca.tables = pl.tables; ca.rec = pl.rec;
-    if (!pl.resamplers.empty()) { ca.rs_res_tab = pl.resamplers[0]->cur_tab; ca.rs_n_res = pl.resamplers[0]->cur_n_res; }
-    if (!pl.samplers.empty()) { ca.smp_res_tab = pl.samplers[0]->cur_tab; ca.smp_n_res = pl.samplers[0]->cur_n_res; }
+    ca.res_tab = ck.res_tab; ca.n_res = ck.n_res;
     for (auto& st : pl.samplers) if (st->cur_n_msgs) ca.smp_msgs = 1;
     if (pl.image.size() <= sizeof(ca.image)) { std::memcpy(ca.image, pl.image.data(), pl.image.size()); ca.image_in_param = 1; }
     ca.flags = pl.d_flags; ca.num_voices = V; ca.frames = T; ca.block_frames = pl.block_frames;
@@ -1751,7 +1728,7 @@ static int enqueue_chunk(fw_processor* p, Plan& pl, const float* d_in, float* d_
         for (uint32_t b : sp.clear) { if (!FW_CUDA(launch_fill(pl.d_pool + (size_t)b * V * T, (size_t)V * T, 0.0f, p->stream))) return FW_PROC_DEVICE_ERROR; p->launches++; }
         int rc = FW_PROC_OK;
         switch (sp.kind) {
-            case Plan::Step::SAMPLER: rc = run_sampler(p, pl, *sp.node, pl.d_srec[sp.sampler_idx], sp.sm0, rows, nb, T); break;
+            case Plan::Step::SAMPLER: rc = run_sampler(p, pl, ck, *sp.node, pl.smp[sp.sampler_idx].rec, sp.sm0, rows, nb); break;
             case Plan::Step::TEMPORAL: rc = run_temporal(p, sp.node.get(), sp.delay.get(), rows, nb, T, zf); break;
             case Plan::Step::REVERB: rc = run_reverb(p, *sp.node, rows, nb, T, zf); break;
             case Plan::Step::PROG:
@@ -1789,7 +1766,7 @@ static int enqueue_chunk(fw_processor* p, Plan& pl, const float* d_in, float* d_
                 ra.out_vstride = ovs; ra.n_out = no; ra.num_voices = V; ra.frames = T; ra.taps = st.params->rs_taps;
                 uint32_t lg = 0; while ((1u << lg) < st.params->rs_phases) ++lg;
                 ra.phase_shift = 32 - lg;
-                ra.table = st.d_rs_table; ra.pos = st.d_rs_pos; ra.step = st.d_rs_step; ra.flags = st.d_rs_flags; ra.res = st.d_rs_res; ra.res_tab = st.cur_tab;
+                ra.table = st.d_rs_table; ra.pos = st.d_rs_pos; ra.step = st.d_rs_step; ra.flags = st.d_rs_flags; ra.res = st.d_rs_res; ra.res_tab = ck.res_tab;
                 if (!FW_LAUNCH(p, 3, 2, launch_resampler(ra, st.d_rs_pos, p->stream))) return FW_PROC_DEVICE_ERROR;
                 break;
             }
@@ -1819,17 +1796,15 @@ static int enqueue_chunk(fw_processor* p, Plan& pl, const float* d_in, float* d_
 // kernels' run time). Programmatic-dependent-launch edges are kept by the capture.
 static int run_chunk(fw_processor* p, Plan& pl, const float* d_in, float* d_out, const Chunk& ck, bool steady) {
     if (!steady || !pl.graphable || p->graphs_off || p->profiling || p->world > 1 || ck.zero_first) return enqueue_chunk(p, pl, d_in, d_out, ck);
-    const ResDesc* res_tab = pl.samplers.empty() ? nullptr : pl.samplers[0]->cur_tab;
-    const uint32_t n_res = pl.samplers.empty() ? 0u : pl.samplers[0]->cur_n_res;
     fw_processor::GraphEntry* e = nullptr; fw_processor::GraphEntry* lru = &p->graphs[0];
     for (auto& g : p->graphs) {
-        if (g.plan == &pl && g.d_in == d_in && g.d_out == d_out && g.t0 == ck.t0 && g.Tc == ck.Tc && g.Tfull == ck.Tfull && g.res_tab == res_tab && g.n_res == n_res) { e = &g; break; }
+        if (g.plan == &pl && g.d_in == d_in && g.d_out == d_out && g.t0 == ck.t0 && g.Tc == ck.Tc && g.Tfull == ck.Tfull && g.res_tab == ck.res_tab && g.n_res == ck.n_res) { e = &g; break; }
         if (g.stamp < lru->stamp) lru = &g;
     }
     if (!e) {  // first sight: remember the key, run normally
         e = lru;
         if (e->exec) { cudaGraphExecDestroy(e->exec); e->exec = nullptr; }
-        e->plan = &pl; e->d_in = d_in; e->d_out = d_out; e->t0 = ck.t0; e->Tc = ck.Tc; e->Tfull = ck.Tfull; e->res_tab = res_tab; e->n_res = n_res; e->seen = 0;
+        e->plan = &pl; e->d_in = d_in; e->d_out = d_out; e->t0 = ck.t0; e->Tc = ck.Tc; e->Tfull = ck.Tfull; e->res_tab = ck.res_tab; e->n_res = ck.n_res; e->seen = 0;
     }
     e->stamp = ++p->graph_stamp;
     if (e->exec) {
@@ -1896,7 +1871,6 @@ static int proc_call(fw_processor* p, const float* d_in, float* d_out, uint32_t 
         }
     }
     const uint32_t F = p->max_block_frames, n_blocks = (T + F - 1) / F;
-    p->first_epoch_of_call = p->call_epoch + 1;
     uint32_t b = 0; size_t next_cmd = 0;  // pend[next_cmd..) have block >= b
     int rc = FW_PROC_OK;
     while (b < n_blocks) {
@@ -1904,11 +1878,6 @@ static int proc_call(fw_processor* p, const float* d_in, float* d_out, uint32_t 
         if (!p->running) { silence_from(b * F); rc = FW_PROC_DROP_PROCESSOR; break; }        // :150-155
         Plan& pl = *p->plan;
         if (n_in != pl.c_in || n_out != pl.c_out) { g_dev_err = "channel counts do not match the compiled graph"; return FW_PROC_BAD_ARGS; }
-        if (b == 0 && !pl.resamplers.empty()) {  // pin the resource table the resamplers read during this call
-            const ResDesc* tab; uint32_t n_res;
-            pl.resamplers[0]->res_table->snapshot(&tab, &n_res);
-            for (auto& st : pl.resamplers) { st->cur_tab = tab; st->cur_n_res = n_res; }
-        }
         while (next_cmd < p->pend_n && p->pend[next_cmd].block < b) ++next_cmd;
         const bool have_cmds = next_cmd < p->pend_n && p->pend[next_cmd].block == b;
         if (have_cmds || !pl.samplers.empty()) { if (!apply_commands(p, pl, b)) return FW_PROC_DEVICE_ERROR; }
@@ -1916,7 +1885,10 @@ static int proc_call(fw_processor* p, const float* d_in, float* d_out, uint32_t 
         uint32_t b_end = std::min(n_blocks, b + pl.chunk_blocks);
         if (nc < p->pend_n && p->pend[nc].block < b_end) b_end = p->pend[nc].block;          // the next timed command splits the call
         next_cmd = nc;
-        Chunk ck{b * F, std::min(T, b_end * F) - b * F, T, 0};
+        Chunk ck{b * F, std::min(T, b_end * F) - b * F, T, 0, nullptr, 0};
+        // one snapshot of the resource table for every sampler and resampler of the chunk; it holds every handle they use (the main
+        // thread checks a handle against the table before it sends it, and the table only grows)
+        if (pl.res) pl.res->snapshot(&ck.res_tab, &ck.n_res);
         if (p->pending_zero_first) { ck.zero_first = std::min(pl.block_frames, ck.Tc); p->pending_zero_first = false; }  // Q11
         bool steady = true;  // no sampler message rides in this chunk's control arguments (stores and uploads precede the chunk: they do not change it)
         for (auto& st : pl.samplers) if (st->cur_n_msgs) steady = false;
@@ -1944,90 +1916,89 @@ int fw_processor_process_planar_device(fw_processor* p, const float* d_in, float
     return proc_call(p, d_in, d_out, n_in, n_out, frames);
 }
 
-// error word of the plan: (chunk epoch << 4) | code, written by the control kernel (1: record budget) or the exchange (2: peer time-out)
-static int check_device_error(fw_processor* p) {
+// error word of the plan: (chunk epoch << 4) | code, written by the control kernel (1: record budget) or the exchange (2: peer time-out);
+// an error counts when it comes from a chunk of epoch since_epoch or later
+static int check_device_error(fw_processor* p, uint32_t since_epoch) {
     if (!p->plan) return 0;
     const uint32_t e = *p->h_err;
-    if ((e & 15u) == 0 || ((e >> 4) != kGraphEpoch && (int32_t)((e >> 4) - (p->first_epoch_of_call & 0x0fffffffu)) < 0)) return 0;
+    if ((e & 15u) == 0 || ((e >> 4) != kGraphEpoch && (int32_t)((e >> 4) - (since_epoch & 0x0fffffffu)) < 0)) return 0;
     if ((e >> 4) == kGraphEpoch) cudaMemsetAsync(p->plan->rec.error, 0, 4, p->stream);  // a replayed chunk cannot stamp its epoch: report once, then clear
     g_dev_err = (e & 15u) == 2 ? "master-bus exchange timed out waiting for a peer rank" : "control pass overflowed its transient-block budget (a gain jump beyond 10000 %?)";
     publish_error();
     return FW_PROC_DEVICE_ERROR;
 }
 
-int fw_processor_process_planar(fw_processor* p, const float* in, float* out, uint32_t n_in, uint32_t n_out, uint64_t frames, double stream_time_secs, uint32_t stream_status, uint64_t* out_mask) {
-    if (!p) return FW_PROC_BAD_ARGS;
+// One call on host buffers, in host chunks of at most max_call_frames (the staging buffers were sized for that at activate): per host
+// chunk, stage_in(t0, Tc) puts the caller's frames [t0, t0 + Tc) into d_in, proc_call runs them and stage_out(t0, Tc, rc) returns
+// d_out to the caller. After a drop, zero_rest(t0) zeroes the caller's output from frame t0 on. One synchronise at the end, then the
+// error word is checked for every chunk of the call and the graph_out silence mask goes to out_mask (when not null).
+extern "C++" {  // a template inside the C ABI block
+template <class StageIn, class StageOut, class ZeroRest>
+static int host_call(fw_processor* p, uint32_t n_in, uint32_t n_out, uint64_t frames, double stream_time_secs, uint32_t stream_status, uint64_t* out_mask,
+                     StageIn&& stage_in, StageOut&& stage_out, ZeroRest&& zero_rest) {
     p->cur_stream_time = stream_time_secs; p->cur_stream_status = stream_status;
     cudaSetDevice(p->device);
-    const uint32_t V = p->num_voices;
-    const size_t in_rows = (size_t)V * n_in, out_rows = (size_t)(p->bus ? 1 : V) * n_out;
-    if (out_mask) *out_mask = 0;
     if (n_in != p->n_in || n_out != p->n_out) { g_dev_err = "channel counts do not match the activated stream"; return FW_PROC_BAD_ARGS; }
+    const uint32_t V = p->num_voices, since_epoch = p->call_epoch + 1;
     int rc = FW_PROC_OK;
     uint64_t t0 = 0;
-    const uint32_t first_epoch = p->call_epoch + 1;
-    do {  // host chunks of at most max_call_frames: the staging buffers were sized for that at activate
+    do {
         const uint64_t Tc = std::min<uint64_t>(frames - t0, p->max_call_frames);
-        if (in_rows && Tc && !FW_CUDA(cudaMemcpy2DAsync(p->d_in, Tc * 4, in + t0, frames * 4, Tc * 4, in_rows, cudaMemcpyHostToDevice, p->stream))) return FW_PROC_DEVICE_ERROR;
+        if (!stage_in(t0, Tc)) return FW_PROC_DEVICE_ERROR;
         rc = proc_call(p, p->d_in, p->d_out, n_in, n_out, Tc);
         if (rc < 0) return rc;
         join_side(p);
-        if (out_rows && Tc && !FW_CUDA(cudaMemcpy2DAsync(out + t0, frames * 4, p->d_out, Tc * 4, Tc * 4, out_rows, cudaMemcpyDeviceToHost, p->stream))) return FW_PROC_DEVICE_ERROR;
+        if (!stage_out(t0, Tc, rc)) return FW_PROC_DEVICE_ERROR;
         t0 += Tc;
     } while (t0 < frames && rc == FW_PROC_OK);
-    if (rc == FW_PROC_DROP_PROCESSOR && t0 < frames) for (size_t r = 0; r < out_rows; ++r) std::memset(out + r * frames + t0, 0, (frames - t0) * 4);
+    if (rc == FW_PROC_DROP_PROCESSOR && t0 < frames) zero_rest(t0);
     const bool ran = rc == FW_PROC_OK && p->plan && frames > 0;
     if (ran) {
-        cudaMemcpyAsync(p->h_masks, p->plan->rec.gout_mask, sizeof(uint64_t) * V, cudaMemcpyDeviceToHost, p->stream);
+        if (out_mask) cudaMemcpyAsync(p->h_masks, p->plan->rec.gout_mask, sizeof(uint64_t) * V, cudaMemcpyDeviceToHost, p->stream);
         cudaMemcpyAsync(p->h_err, p->plan->rec.error, sizeof(uint32_t), cudaMemcpyDeviceToHost, p->stream);
     }
     if (!FW_CUDA(cudaStreamSynchronize(p->stream))) return FW_PROC_DEVICE_ERROR;
     if (ran) {
-        p->first_epoch_of_call = first_epoch;
-        if (check_device_error(p)) return FW_PROC_DEVICE_ERROR;
+        if (check_device_error(p, since_epoch)) return FW_PROC_DEVICE_ERROR;
         if (out_mask) *out_mask = p->bus ? bus_mask_from(p->h_masks, V, n_out) : p->h_masks[0];
     }
     return rc;
 }
+}  // extern "C++"
+
+int fw_processor_process_planar(fw_processor* p, const float* in, float* out, uint32_t n_in, uint32_t n_out, uint64_t frames, double stream_time_secs, uint32_t stream_status, uint64_t* out_mask) {
+    if (!p) return FW_PROC_BAD_ARGS;
+    if (out_mask) *out_mask = 0;
+    const size_t in_rows = (size_t)p->num_voices * n_in, out_rows = (size_t)(p->bus ? 1 : p->num_voices) * n_out;
+    return host_call(p, n_in, n_out, frames, stream_time_secs, stream_status, out_mask,
+        [&](uint64_t t0, uint64_t Tc) { return !in_rows || !Tc || FW_CUDA(cudaMemcpy2DAsync(p->d_in, Tc * 4, in + t0, frames * 4, Tc * 4, in_rows, cudaMemcpyHostToDevice, p->stream)); },
+        [&](uint64_t t0, uint64_t Tc, int) { return !out_rows || !Tc || FW_CUDA(cudaMemcpy2DAsync(out + t0, frames * 4, p->d_out, Tc * 4, Tc * 4, out_rows, cudaMemcpyDeviceToHost, p->stream)); },
+        [&](uint64_t t0) { for (size_t r = 0; r < out_rows; ++r) std::memset(out + r * frames + t0, 0, (frames - t0) * 4); });
+}
 
 int fw_processor_process_interleaved(fw_processor* p, const float* in, float* out, uint32_t n_in, uint32_t n_out, uint64_t frames, double stream_time_secs, uint32_t stream_status) {
     if (!p) return FW_PROC_BAD_ARGS;
-    p->cur_stream_time = stream_time_secs; p->cur_stream_status = stream_status;
-    cudaSetDevice(p->device);
     const uint32_t V = p->num_voices, Vo = p->bus ? 1 : V;
-    if (n_in != p->n_in || n_out != p->n_out) { g_dev_err = "channel counts do not match the activated stream"; return FW_PROC_BAD_ARGS; }
-    int rc = FW_PROC_OK;
-    uint64_t t0 = 0;
-    const uint32_t first_epoch = p->call_epoch + 1;
-    do {
-        const uint64_t Tc = std::min<uint64_t>(frames - t0, p->max_call_frames);
-        if (n_in && Tc) {  // voice v's frames [t0, t0 + Tc) are one contiguous run of Tc * n_in floats
-            if (!FW_CUDA(cudaMemcpy2DAsync(p->d_inter, Tc * n_in * 4, in + t0 * n_in, frames * n_in * 4, Tc * n_in * 4, V, cudaMemcpyHostToDevice, p->stream))) return FW_PROC_DEVICE_ERROR;
-            if (!FW_CUDA(launch_deinterleave(p->d_inter, p->d_in, V, n_in, (uint32_t)Tc, p->stream))) return FW_PROC_DEVICE_ERROR;
+    return host_call(p, n_in, n_out, frames, stream_time_secs, stream_status, nullptr,
+        [&](uint64_t t0, uint64_t Tc) {  // voice v's frames [t0, t0 + Tc) are one contiguous run of Tc * n_in floats
+            if (!n_in || !Tc) return true;
+            if (!FW_CUDA(cudaMemcpy2DAsync(p->d_inter, Tc * n_in * 4, in + t0 * n_in, frames * n_in * 4, Tc * n_in * 4, V, cudaMemcpyHostToDevice, p->stream))) return false;
+            if (!FW_CUDA(launch_deinterleave(p->d_inter, p->d_in, V, n_in, (uint32_t)Tc, p->stream))) return false;
             p->launches++;
-        }
-        rc = proc_call(p, p->d_in, p->d_out, n_in, n_out, Tc);
-        if (rc < 0) return rc;
-        join_side(p);
-        if (n_out && Tc) {
-            const bool ran = rc == FW_PROC_OK && p->plan;
+            return true;
+        },
+        [&](uint64_t t0, uint64_t Tc, int rc) {
+            if (!n_out || !Tc) return true;
             const uint64_t* masks = nullptr;
-            if (ran) {
+            if (rc == FW_PROC_OK && p->plan) {
                 if (p->bus) { launch_bus_mask(p->plan->rec.gout_mask, V, n_out, p->plan->d_bus_mask, p->stream); p->launches++; masks = p->plan->d_bus_mask; }
                 else masks = p->plan->rec.gout_mask;
             }
-            if (!FW_CUDA(launch_interleave(p->d_out, p->d_inter, masks, Vo, n_out, (uint32_t)Tc, p->max_block_frames, p->stream))) return FW_PROC_DEVICE_ERROR;
+            if (!FW_CUDA(launch_interleave(p->d_out, p->d_inter, masks, Vo, n_out, (uint32_t)Tc, p->max_block_frames, p->stream))) return false;
             p->launches++;
-            if (!FW_CUDA(cudaMemcpy2DAsync(out + t0 * n_out, frames * n_out * 4, p->d_inter, Tc * n_out * 4, Tc * n_out * 4, Vo, cudaMemcpyDeviceToHost, p->stream))) return FW_PROC_DEVICE_ERROR;
-        }
-        t0 += Tc;
-    } while (t0 < frames && rc == FW_PROC_OK);
-    if (rc == FW_PROC_DROP_PROCESSOR && t0 < frames) for (size_t v = 0; v < Vo; ++v) std::memset(out + (v * frames + t0) * n_out, 0, (frames - t0) * n_out * 4);
-    const bool ran = rc == FW_PROC_OK && p->plan && frames > 0;
-    if (ran) cudaMemcpyAsync(p->h_err, p->plan->rec.error, sizeof(uint32_t), cudaMemcpyDeviceToHost, p->stream);
-    if (!FW_CUDA(cudaStreamSynchronize(p->stream))) return FW_PROC_DEVICE_ERROR;
-    if (ran) { p->first_epoch_of_call = first_epoch; if (check_device_error(p)) return FW_PROC_DEVICE_ERROR; }
-    return rc;
+            return FW_CUDA(cudaMemcpy2DAsync(out + t0 * n_out, frames * n_out * 4, p->d_inter, Tc * n_out * 4, Tc * n_out * 4, Vo, cudaMemcpyDeviceToHost, p->stream));
+        },
+        [&](uint64_t t0) { for (size_t v = 0; v < Vo; ++v) std::memset(out + (v * frames + t0) * n_out, 0, (frames - t0) * n_out * 4); });
 }
 
 void fw_processor_free(fw_processor* p) {  // Drop processor.rs:251-263
@@ -2060,7 +2031,7 @@ int fw_processor_sync(fw_processor* p) {
     cudaSetDevice(p->device);
     join_side(p);
     if (!FW_CUDA(cudaStreamSynchronize(p->stream))) return -1;
-    if (p->plan) { cudaMemcpy(p->h_err, p->plan->rec.error, 4, cudaMemcpyDeviceToHost); p->first_epoch_of_call = p->synced_epoch + 1; p->synced_epoch = p->call_epoch; if (check_device_error(p)) return -1; }
+    if (p->plan) { cudaMemcpy(p->h_err, p->plan->rec.error, 4, cudaMemcpyDeviceToHost); const uint32_t since = p->synced_epoch + 1; p->synced_epoch = p->call_epoch; if (check_device_error(p, since)) return -1; }
     return 0;
 }
 int fw_processor_event_record(fw_processor* p, int slot) { if (slot < 0 || slot > 3) return -1; cudaSetDevice(p->device); join_side(p); return FW_CUDA(cudaEventRecord(p->ev[slot], p->stream)) ? 0 : -1; }
