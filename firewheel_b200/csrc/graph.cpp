@@ -6,36 +6,30 @@
 
 namespace fw {
 
-const char* node_debug_name(uint32_t kind) {
-    switch (kind) {
-        case FW_NODE_DUMMY: return "dummy";                    // dummy.rs:8
-        case FW_NODE_VOLUME: return "volume";                  // volume.rs:43
-        case FW_NODE_SUM: return "sum";                        // sum.rs:7
-        case FW_NODE_MONO_TO_STEREO: return "mono_to_stereo";  // mono_to_stereo.rs:7
-        case FW_NODE_STEREO_TO_MONO: return "stereo_to_mono";  // stereo_to_mono.rs:7
-        case FW_NODE_HARD_CLIP: return "hard_clip";            // hard_clip.rs:17
-        case FW_NODE_PAN: return "pan";
-        case FW_NODE_BIQUAD: return "biquad";
-        case FW_NODE_DELAY: return "delay";
-        case FW_NODE_CONV_REVERB: return "conv_reverb";
-        case FW_NODE_SVF: return "svf";
-        case FW_NODE_RESAMPLER: return "resampler";
-        case FW_NODE_SAMPLER: return "beep_test";              // Q8: sampler.rs:186 really says that
-        case FW_NODE_CUSTOM: return "custom";                  // the context reports the plugin's own debug_name()
-        default: return "unknown";
-    }
-}
+// One row per fw_node_kind in kind order, then the row of an unknown kind. info: {min in, max in, min out, max out, updates}; op: {on,
+// kind, c_in, c_out, pairs, mask, fuses}, {} when the node is not a chain op; chan, vary, res: per_channel_state, call_varying, reads_resources.
+static constexpr NodeKind kNodeKinds[] = {
+    //kind                   name              info               coeffs targets                                     step            op                                        chan   vary   res
+    {FW_NODE_DUMMY,          "dummy",          {0, 64, 0, 64, 0}, 0,     {},                                         STEP_PROG,      {},                                       false, false, false},  // dummy.rs:8-18
+    {FW_NODE_VOLUME,         "volume",         {1, 64, 1, 64, 0}, 0,     {&NodeParams::raw_gain},                    STEP_PROG,      {true, OP_GAIN, 2, 2, true, true, true},  false, false, false},  // volume.rs:43-54
+    {FW_NODE_SUM,            "sum",            {1, 64, 1, 64, 0}, 0,     {},                                         STEP_SUM,       {},                                       false, false, false},  // sum.rs:7
+    {FW_NODE_MONO_TO_STEREO, "mono_to_stereo", {1, 1, 2, 2, 0},   0,     {},                                         STEP_PROG,      {true, OP_M2S, 1, 2, false, true, false}, false, false, false},  // mono_to_stereo.rs:7-18
+    {FW_NODE_STEREO_TO_MONO, "stereo_to_mono", {2, 2, 1, 1, 0},   0,     {},                                         STEP_PROG,      {true, OP_S2M, 2, 1, false, true, false}, false, false, false},  // stereo_to_mono.rs:7-18
+    {FW_NODE_HARD_CLIP,      "hard_clip",      {1, 64, 1, 64, 0}, 0,     {},                                         STEP_PROG,      {true, OP_CLIP, 2, 2, true, true, false}, false, false, false},  // hard_clip.rs:17
+    {FW_NODE_PAN,            "pan",            {2, 2, 2, 2, 0},   0,     {&NodeParams::gain_l, &NodeParams::gain_r}, STEP_PROG,      {true, OP_PAN, 2, 2, false, false, true}, false, false, false},
+    {FW_NODE_BIQUAD,         "biquad",         {1, 64, 1, 64, 0}, 5,     {},                                         STEP_TEMPORAL,  {},                                       true,  false, false},
+    {FW_NODE_DELAY,          "delay",          {1, 64, 1, 64, 0}, 0,     {},                                         STEP_TEMPORAL,  {},                                       true,  true,  false},
+    {FW_NODE_CONV_REVERB,    "conv_reverb",    {1, 64, 1, 64, 0}, 0,     {},                                         STEP_REVERB,    {},                                       true,  true,  false},
+    {FW_NODE_SAMPLER,        "beep_test",      {0, 0, 1, 64, 1},  0,     {&NodeParams::raw_gain},                    STEP_SAMPLER,   {},                                       false, false, true},   // Q8: sampler.rs:186 really says that; sampler.rs:189-196
+    {FW_NODE_SVF,            "svf",            {1, 64, 1, 64, 0}, 6,     {},                                         STEP_TEMPORAL,  {},                                       true,  false, false},
+    {FW_NODE_RESAMPLER,      "resampler",      {0, 0, 1, 64, 0},  0,     {},                                         STEP_RESAMPLER, {},                                       false, true,  true},
+    {FW_NODE_CUSTOM,         "custom",         {1, 64, 1, 64, 0}, 0,     {},                                         STEP_CUSTOM,    {},                                       false, true,  false},  // the context reports the plugin's own name and info
+    {FW_NODE_CUSTOM + 1,     "unknown",        {1, 64, 1, 64, 0}, 0,     {},                                         STEP_PROG,      {},                                       false, false, false},
+};
+constexpr bool rows_in_kind_order() { for (uint32_t k = 0; k < sizeof(kNodeKinds) / sizeof(kNodeKinds[0]); ++k) if (kNodeKinds[k].kind != k) return false; return true; }
+static_assert(sizeof(kNodeKinds) / sizeof(kNodeKinds[0]) == FW_NODE_CUSTOM + 2 && rows_in_kind_order(), "one row per fw_node_kind, then the unknown row");
 
-void node_supported_ports(uint32_t kind, uint32_t* mi, uint32_t* xi, uint32_t* mo, uint32_t* xo) {
-    switch (kind) {
-        case FW_NODE_DUMMY: *mi = 0; *xi = 64; *mo = 0; *xo = 64; break;          // dummy.rs:12-18
-        case FW_NODE_MONO_TO_STEREO: *mi = 1; *xi = 1; *mo = 2; *xo = 2; break;   // mono_to_stereo.rs:10-18
-        case FW_NODE_STEREO_TO_MONO: *mi = 2; *xi = 2; *mo = 1; *xo = 1; break;   // stereo_to_mono.rs:10-18
-        case FW_NODE_PAN: *mi = 2; *xi = 2; *mo = 2; *xo = 2; break;
-        case FW_NODE_SAMPLER: case FW_NODE_RESAMPLER: *mi = 0; *xi = 0; *mo = 1; *xo = 64; break;         // sampler.rs:189-196
-        default: *mi = 1; *xi = 64; *mo = 1; *xo = 64; break;                      // volume.rs:46-54 et al.
-    }
-}
+const NodeKind& node_kind(uint32_t kind) { return kNodeKinds[kind <= FW_NODE_CUSTOM ? kind : FW_NODE_CUSTOM + 1]; }
 
 std::string node_check_activation(const NodeParams& p, uint32_t ni, uint32_t no) {
     auto got = [&] { return "Got num_inputs: " + std::to_string(ni) + ", num_outputs: " + std::to_string(no); };

@@ -23,6 +23,7 @@
 #include <vector>
 
 #include "../../include/fw_b200.h"
+#include "plan.hpp"
 
 namespace fw {
 
@@ -130,12 +131,33 @@ struct NodeParams {
     std::vector<uint16_t> smp_pending;     // messages queued per voice since the stream side last drained (ring capacity 128, sampler.rs:14)
     std::vector<uint32_t> smp_pending_epoch;  // drain epoch `smp_pending[v]` was counted in
 };
-// floats per stage in NodeParams::coeffs: 5 for a biquad, 6 for an SVF, 0 for a node without a coefficient table
-inline uint32_t coeff_width(uint32_t kind) { return kind == FW_NODE_BIQUAD ? 5 : kind == FW_NODE_SVF ? 6 : 0; }
 
-const char* node_debug_name(uint32_t kind);
-// AudioNodeInfo per kind (node.rs:57-79 as filled in by each basic node)
-void node_supported_ports(uint32_t kind, uint32_t* min_in, uint32_t* max_in, uint32_t* min_out, uint32_t* max_out);
+// The data-plane step that runs a node (Plan::Step in runtime.cu)
+enum StepKind : uint8_t { STEP_PROG, STEP_SAMPLER, STEP_TEMPORAL, STEP_REVERB, STEP_SUM, STEP_RESAMPLER, STEP_CUSTOM };
+
+// What a node kind is, for the graph, the activation and the device lowering: one row per fw_node_kind (graph.cpp).
+struct NodeKind {
+    uint32_t kind; const char* name;  // name: the debug_name the graph reports
+    fw_audio_node_info info;          // AudioNodeInfo (node.rs:57-79 as filled in by each basic node); out_silence_rule is unused
+    uint32_t coeff_width;             // floats per stage in NodeParams::coeffs (0: no coefficient table)
+    using Target = std::vector<float> NodeParams::*;
+    Target target[2];                 // the target arrays of the node's smoothed parameters, in smoother order (null: none)
+    StepKind step;                    // the data-plane step that runs the node (a 1-port SumNode is a copy: a PROG step)
+    struct {
+        bool on; ChainOpKind kind;    // the node is one chain op of this kind
+        uint32_t c_in, c_out;         // the op's program widths in the generic lowering
+        bool pairs;                   // the generic lowering runs the op per channel pair
+        bool mask;                    // the op's body branches on the input silence mask (a stereo Volume's does not)
+        bool fuses;                   // a stereo node joins fused runs of the generic lowering
+    } op;
+    bool per_channel_state;           // device state sized by the port count: the node is activated again when the count changes
+    bool call_varying;                // kernel arguments change from call to call (cursors, positions, plugin calls): no graph replay
+    bool reads_resources;             // reads the context's sample resources
+};
+// The row of `kind`; an unknown kind's row for an out-of-range value
+const NodeKind& node_kind(uint32_t kind);
+inline uint32_t coeff_width(uint32_t kind) { return node_kind(kind).coeff_width; }
+
 // AudioNode::activate argument checks (volume.rs:63-65, sum.rs:27-29, hard_clip.rs:37-39, ours). "" => Ok.
 std::string node_check_activation(const NodeParams& p, uint32_t num_inputs, uint32_t num_outputs);
 

@@ -125,7 +125,7 @@ struct NodeDeviceState {
     DevMem mem;  // every buffer below
     uint32_t kind = 0, V = 0, n_sm = 0;
     std::shared_ptr<NodeParams> params;
-    float* d_target[2] = {nullptr, nullptr};      // volume: raw_gain; pan: gain_l, gain_r
+    float* d_target[2] = {nullptr, nullptr};      // the smoothed parameters' targets (NodeKind::target)
     float* sm_input[2] = {nullptr, nullptr};
     float* sm_last[2] = {nullptr, nullptr};
     uint32_t* sm_status[2] = {nullptr, nullptr};
@@ -158,14 +158,14 @@ struct NodeDeviceState {
         }
         if (ev_staged) cudaEventDestroy(ev_staged);
     }
-    const std::vector<float>& host_target(int i) const { return (kind == FW_NODE_VOLUME || kind == FW_NODE_SAMPLER) ? params->raw_gain : (i == 0 ? params->gain_l : params->gain_r); }
     // ParamSmoother::new(val): input = last_output = val, Inactive (smoother.rs:93-112; volume.rs:67-75)
     bool create() {
-        n_sm = (kind == FW_NODE_VOLUME || kind == FW_NODE_SAMPLER) ? 1 : kind == FW_NODE_PAN ? 2 : 0;
+        const NodeKind& nk = node_kind(kind);
+        n_sm = nk.target[1] ? 2 : nk.target[0] ? 1 : 0;
         for (uint32_t i = 0; i < n_sm; ++i) {
             d_target[i] = mem.dev<float>(V); sm_input[i] = mem.dev<float>(V); sm_last[i] = mem.dev<float>(V); sm_status[i] = mem.dev<uint32_t>(V);
             if (!mem.ok()) return false;
-            const float* h = host_target(i).data();
+            const float* h = ((*params).*nk.target[i]).data();
             if (!FW_CUDA(cudaMemcpy(d_target[i], h, V * 4, cudaMemcpyHostToDevice))) return false;
             if (!FW_CUDA(cudaMemcpy(sm_input[i], h, V * 4, cudaMemcpyHostToDevice))) return false;
             if (!FW_CUDA(cudaMemcpy(sm_last[i], h, V * 4, cudaMemcpyHostToDevice))) return false;
@@ -262,7 +262,7 @@ struct Plan {
     enum Space : uint8_t { CALLER_IN, CALLER_OUT, POOL, SCRATCH };
     struct Operand { Space space; uint32_t index, C; };
     struct Step {
-        enum Kind : uint8_t { PROG, SAMPLER, TEMPORAL, REVERB, SUM, RESAMPLER, CUSTOM } kind = PROG;
+        StepKind kind = STEP_PROG;
         // node: the sampler, the biquad or SVF of a temporal step (none: a lone delay), the reverb, resampler or custom node; delay: a
         // temporal step's delay line
         std::shared_ptr<NodeDeviceState> node, delay;
@@ -406,17 +406,12 @@ struct ProfScope {  // brackets the launches of one kernel class with a pair of 
 // =============================================================================================
 // lowering: schedule -> control tables + fused chain program
 // =============================================================================================
-// The chain op of a pointwise node kind; false for every other kind. sm0: the node's first smoother; threshold_gain: HardClip's threshold.
-static bool chain_op(uint32_t kind, int sm0, float threshold_gain, ChainOp* op) {
-    *op = ChainOp{}; op->sm0 = op->sm1 = -1;
-    switch (kind) {
-        case FW_NODE_VOLUME: op->kind = OP_GAIN; op->sm0 = sm0; return true;
-        case FW_NODE_PAN: op->kind = OP_PAN; op->sm0 = sm0; op->sm1 = sm0 + 1; return true;
-        case FW_NODE_HARD_CLIP: op->kind = OP_CLIP; op->f0 = threshold_gain; return true;
-        case FW_NODE_MONO_TO_STEREO: op->kind = OP_M2S; return true;
-        case FW_NODE_STEREO_TO_MONO: op->kind = OP_S2M; return true;
-        default: return false;
-    }
+// The chain op of a node whose kind has one (NodeKind::op.on). sm0: the node's first smoother; its second, if any, is sm0 + 1.
+static ChainOp chain_op(const NodeParams& np, int sm0) {
+    const NodeKind& nk = node_kind(np.kind);
+    ChainOp op{}; op.kind = nk.op.kind; op.sm0 = nk.target[0] ? sm0 : -1; op.sm1 = nk.target[1] ? sm0 + 1 : -1;
+    if (nk.op.kind == OP_CLIP) op.f0 = np.threshold_gain;
+    return op;
 }
 
 // Control tables (one CtlNode per scheduled node, the smoothers, the sampler and resampler transport state) and the node states of
@@ -506,7 +501,7 @@ static bool lower_chain(const Schedule& s, const std::vector<int>& sm_of_node, b
     std::vector<Plan::Step>& steps = plan->steps;
     uint32_t width = (uint32_t)gin.out.size();
     // a stage of `width` channels in and out (the space and index of its operands are set at the end)
-    auto stage = [&](Plan::Step::Kind kind, const std::shared_ptr<NodeDeviceState>& node) {
+    auto stage = [&](StepKind kind, const std::shared_ptr<NodeDeviceState>& node) {
         Plan::Step sp; sp.kind = kind; sp.node = node;
         sp.in = {Plan::Operand{Plan::SCRATCH, 0, width}}; sp.out = sp.in;
         steps.push_back(std::move(sp));
@@ -516,7 +511,7 @@ static bool lower_chain(const Schedule& s, const std::vector<int>& sm_of_node, b
     if (width == 0 && n >= 3 && plan->nodes[1].kind == FW_NODE_SAMPLER && s.nodes[1].in.empty() && s.nodes[1].out.size() >= 1 && s.nodes[1].out.size() <= 2) {
         // no stream inputs: a SamplerNode heads the chain (BASELINE config 5: sampler -> gain -> pan -> ... -> bus)
         width = (uint32_t)s.nodes[1].out.size();
-        stage(Plan::Step::SAMPLER, plan->states[1]);
+        stage(STEP_SAMPLER, plan->states[1]);
         steps.back().in.clear(); steps.back().sm0 = sm_of_node[1]; steps.back().sampler_idx = plan->nodes[1].sm1;
         prev = s.nodes[1].id; first = 2;
     }
@@ -528,7 +523,7 @@ static bool lower_chain(const Schedule& s, const std::vector<int>& sm_of_node, b
     };
     ChainProgram cur{}; cur.c_in = width;  // the pointwise stage being accumulated
     auto close_pointwise = [&](bool force) {
-        if (cur.n_ops > 0 || force) { cur.c_out = width; stage(Plan::Step::PROG, nullptr); steps.back().prog = cur; steps.back().in[0].C = cur.c_in; }
+        if (cur.n_ops > 0 || force) { cur.c_out = width; stage(STEP_PROG, nullptr); steps.back().prog = cur; steps.back().in[0].C = cur.c_in; }
         cur = ChainProgram{}; cur.c_in = width;
     };
     for (size_t i = first; i + 1 < n; ++i) {
@@ -537,15 +532,16 @@ static bool lower_chain(const Schedule& s, const std::vector<int>& sm_of_node, b
         if (!fed_by_prev(sn, width)) { *why = "voice graph is not a linear port-to-port chain"; return false; }
         if (sn.out.size() < 1 || sn.out.size() > 2) { *why = "the fused chain supports 1 or 2 channels"; return false; }
         const uint32_t kind = np.kind;
-        if (kind == FW_NODE_CONV_REVERB || kind == FW_NODE_SVF || kind == FW_NODE_BIQUAD || kind == FW_NODE_DELAY) {
+        const NodeKind& nk = node_kind(kind);
+        if (nk.step == STEP_TEMPORAL || nk.step == STEP_REVERB) {
             const std::shared_ptr<NodeDeviceState>& st = plan->states[i];
             // a delay directly after a biquad joins its pass; anything else opens a new stage
-            if (kind == FW_NODE_DELAY && !steps.empty() && steps.back().kind == Plan::Step::TEMPORAL && !steps.back().delay &&
+            if (kind == FW_NODE_DELAY && !steps.empty() && steps.back().kind == STEP_TEMPORAL && !steps.back().delay &&
                 steps.back().node && steps.back().node->kind == FW_NODE_BIQUAD && cur.n_ops == 0) {
                 steps.back().delay = st;
             } else {
                 close_pointwise(false);
-                stage(kind == FW_NODE_CONV_REVERB ? Plan::Step::REVERB : Plan::Step::TEMPORAL, kind == FW_NODE_DELAY ? nullptr : st);
+                stage(nk.step, kind == FW_NODE_DELAY ? nullptr : st);
                 if (kind == FW_NODE_DELAY) steps.back().delay = st;
             }
             prev = sn.id;
@@ -556,15 +552,15 @@ static bool lower_chain(const Schedule& s, const std::vector<int>& sm_of_node, b
             if (sn.in.size() == sn.out.size()) { prev = sn.id; continue; }  // 1-port sum == copy (sum.rs:58-65): no data op
             *why = "SumNode with more than one port inside a voice chain"; return false;
         }
-        ChainOp op;
-        if (!chain_op(kind, sm_of_node[i], np.threshold_gain, &op)) { *why = std::string("node kind '") + node_debug_name(kind) + "' has no device lowering yet"; return false; }
+        if (!nk.op.on) { *why = std::string("node kind '") + nk.name + "' has no device lowering yet"; return false; }
+        const ChainOp op = chain_op(np, sm_of_node[i]);
         if (!prog_push(cur, op)) { close_pointwise(false); prog_push(cur, op); }  // a program reads at most kMaxProgSmoothers smoothers
         width = (uint32_t)sn.out.size();
         prev = sn.id;
     }
     if (!fed_by_prev(gout, width)) { *why = "graph_out is not fed port-to-port by the end of the chain"; return false; }
     // the last stage must be pointwise when the master bus follows it, and a plan is never empty
-    close_pointwise(steps.empty() || (bus && cur.n_ops == 0 && steps.back().kind != Plan::Step::PROG));
+    close_pointwise(steps.empty() || (bus && cur.n_ops == 0 && steps.back().kind != STEP_PROG));
     for (uint32_t si = 0; si < steps.size(); ++si) {
         const bool last = si + 1 == steps.size();
         for (Plan::Operand& o : steps[si].in) o = si == 0 ? Plan::Operand{Plan::CALLER_IN, 0, o.C} : Plan::Operand{Plan::SCRATCH, (si - 1) & 1, o.C};
@@ -594,10 +590,10 @@ static bool lower_generic(const Schedule& s, const std::vector<int>& sm_of_node,
         for (const OutAssign& a : sn.out) sp.out.push_back(Plan::Operand{Plan::POOL, a.buffer, 1});
         if (i == 0) for (uint32_t p = 0; p < sn.out.size(); ++p) sp.in.push_back(Plan::Operand{Plan::CALLER_IN, p, 1});
         if (i + 1 == n && !bus) for (uint32_t p = 0; p < sn.in.size(); ++p) sp.out.push_back(Plan::Operand{Plan::CALLER_OUT, p, 1});
+        const NodeKind& nk = node_kind(kind);
+        sp.kind = kind == FW_NODE_SUM && sn.in.size() == sn.out.size() ? STEP_PROG : nk.step;  // a 1-port SumNode is a copy (sum.rs:58-65)
         // bodies that branch on the input silence mask (see silence_fix_kernel / sum_kernel)
-        const bool needs_mask = !endpoint && ((kind == FW_NODE_CUSTOM) || (!sn.out.empty() &&
-            ((kind == FW_NODE_SUM && sn.in.size() != sn.out.size()) || kind == FW_NODE_HARD_CLIP || (kind == FW_NODE_VOLUME && sn.in.size() != 2) ||
-             kind == FW_NODE_MONO_TO_STEREO || kind == FW_NODE_STEREO_TO_MONO)));
+        const bool needs_mask = !endpoint && (sp.kind == STEP_CUSTOM || (!sn.out.empty() && (sp.kind == STEP_SUM || (nk.op.mask && !(kind == FW_NODE_VOLUME && sn.in.size() == 2)))));
         if (kind == FW_NODE_CUSTOM && !np.custom->vt.process_device) { *why = std::string("custom node '") + np.custom->debug_name + "' has no process_device: it cannot run on the device (there is no CPU fallback)"; return false; }
         if (needs_mask) {
             sp.mask_slot = (int)n_sum_masks; plan->nodes[i].mask_slot = ++n_sum_masks;
@@ -605,26 +601,19 @@ static bool lower_generic(const Schedule& s, const std::vector<int>& sm_of_node,
         if (kind == FW_NODE_DUMMY && !endpoint && !sn.out.empty()) { *why = "a DummyAudioNode inside the graph leaves its outputs stale in the reference (dummy.rs:34-41): not reproducible on the device"; return false; }
         if (kind == FW_NODE_MONO_TO_STEREO && (sn.in.size() != 1 || sn.out.size() != 2)) { *why = "MonoToStereoNode must be 1 -> 2"; return false; }
         if (kind == FW_NODE_STEREO_TO_MONO && (sn.in.size() != 2 || sn.out.size() != 1)) { *why = "StereoToMonoNode must be 2 -> 1"; return false; }
-        // The program: a copy for graph_in, graph_out (both Dummy nodes), a 1-port SumNode (sum.rs:58-65) and a Dummy node inside the
-        // graph, which has no outputs and so launches nothing; else the node's op. It runs per channel pair where the body works channel
-        // by channel, else once for the node; fuse_generic makes a stereo Volume it fuses, or that reads the caller's rows, one launch
-        // too. With a master bus, the bus stage takes graph_out's channels at once.
-        ChainOp op;
-        if (kind == FW_NODE_DUMMY || (kind == FW_NODE_SUM && sn.in.size() == sn.out.size())) {
+        // The program: the node's op, else a copy for graph_in, graph_out (both Dummy nodes), a 1-port SumNode and a Dummy node inside the
+        // graph, which has no outputs and so launches nothing. It runs per channel pair where the body works channel by channel, else once
+        // for the node; fuse_generic makes a stereo Volume it fuses, or that reads the caller's rows, one launch too. With a master bus, the
+        // bus stage takes graph_out's channels at once.
+        if (nk.op.on) {
+            prog_push(sp.prog, chain_op(np, sp.sm0));
+            sp.prog.c_in = nk.op.c_in; sp.prog.c_out = nk.op.c_out; sp.pairs = nk.op.pairs;
+        } else if (sp.kind == STEP_PROG) {
             const bool bus_out = bus && i + 1 == n;
             sp.prog.c_in = sp.prog.c_out = bus_out ? (uint32_t)sn.in.size() : 2u; sp.pairs = !bus_out;
-        } else if (chain_op(kind, sp.sm0, np.threshold_gain, &op)) {
-            prog_push(sp.prog, op);
-            sp.prog.c_in = kind == FW_NODE_MONO_TO_STEREO ? 1u : 2u; sp.prog.c_out = kind == FW_NODE_STEREO_TO_MONO ? 1u : 2u;
-            sp.pairs = kind == FW_NODE_VOLUME || kind == FW_NODE_HARD_CLIP;
-        } else if (kind == FW_NODE_BIQUAD || kind == FW_NODE_SVF || kind == FW_NODE_DELAY) {
-            sp.kind = Plan::Step::TEMPORAL;
-            if (kind == FW_NODE_DELAY) std::swap(sp.node, sp.delay);
-        } else {
-            sp.kind = kind == FW_NODE_SUM ? Plan::Step::SUM : kind == FW_NODE_SAMPLER ? Plan::Step::SAMPLER : kind == FW_NODE_CONV_REVERB ? Plan::Step::REVERB :
-                      kind == FW_NODE_RESAMPLER ? Plan::Step::RESAMPLER : Plan::Step::CUSTOM;
-            if (kind == FW_NODE_SAMPLER) sp.sampler_idx = plan->nodes[i].sm1;
         }
+        if (kind == FW_NODE_DELAY) std::swap(sp.node, sp.delay);
+        if (kind == FW_NODE_SAMPLER) sp.sampler_idx = plan->nodes[i].sm1;
         plan->steps.push_back(std::move(sp));
     }
     plan->rec.n_sum_masks = n_sum_masks;
@@ -642,7 +631,7 @@ static bool lower_generic(const Schedule& s, const std::vector<int>& sm_of_node,
 static void fuse_generic(const Schedule& s, Plan* plan) {
     const size_t n = s.nodes.size();
     std::vector<Plan::Step>& st = plan->steps;  // one per scheduled node until the end
-    auto kind = [&](size_t i) { return plan->states[i]->kind; };
+    auto nk = [&](size_t i) -> const NodeKind& { return node_kind(plan->states[i]->kind); };
     std::unordered_map<uint64_t, size_t> index_of;
     for (size_t i = 0; i < n; ++i) index_of[s.nodes[i].id.pack()] = i;
     std::vector<std::vector<uint32_t>> n_cons(n);
@@ -654,7 +643,7 @@ static void fuse_generic(const Schedule& s, Plan* plan) {
     }
     auto connected = [&](size_t i) { for (const InAssign& a : s.nodes[i].in) if (a.should_clear) return false; return true; };
     auto stereo_pointwise = [&](size_t i) {
-        return i > 0 && i + 1 < n && (kind(i) == FW_NODE_PAN || kind(i) == FW_NODE_VOLUME) && s.nodes[i].in.size() == 2 && s.nodes[i].out.size() == 2 &&
+        return i > 0 && i + 1 < n && nk(i).op.fuses && s.nodes[i].in.size() == 2 && s.nodes[i].out.size() == 2 &&
                st[i].mask_slot < 0 && connected(i);
     };
     auto fed_only_by = [&](size_t i, size_t j) {  // node i's inputs are node j's outputs, port to port, and nothing else reads them
@@ -669,8 +658,7 @@ static void fuse_generic(const Schedule& s, Plan* plan) {
     // graph_in aliasing: which nodes can read the caller's rows, and is the pool copy still needed
     std::vector<uint32_t> alias_cons(s.nodes[0].out.size(), 0u);
     for (size_t i = 1; i + 1 < n; ++i) {
-        const bool temporal = kind(i) == FW_NODE_BIQUAD || kind(i) == FW_NODE_SVF || kind(i) == FW_NODE_DELAY;
-        if (!(stereo_pointwise(i) || (temporal && connected(i) && !s.nodes[i].in.empty()))) continue;
+        if (!(stereo_pointwise(i) || (nk(i).step == STEP_TEMPORAL && connected(i) && !s.nodes[i].in.empty()))) continue;
         bool all = true;
         for (const InAssign& a : s.nodes[i].in) if (a.producer != s.nodes[0].id || a.producer_port >= alias_cons.size()) all = false;
         if (!all) continue;
@@ -752,7 +740,7 @@ static bool alloc_plan(const fw_ctx* c, Plan* plan, bool pool, std::string* why)
                 plan->smp[i].rec = mem.dev<SmpRec>((size_t)Kc * V); plan->smp[i].last_play = mem.dev<uint32_t>(V);
             }
         }
-        for (auto& sp : plan->steps) if (sp.kind == Plan::Step::CUSTOM) { sp.custom_idx = (int)plan->d_custom_masks.size(); plan->d_custom_masks.push_back(mem.dev<uint64_t>((size_t)Kc * V)); }
+        for (auto& sp : plan->steps) if (sp.kind == STEP_CUSTOM) { sp.custom_idx = (int)plan->d_custom_masks.size(); plan->d_custom_masks.push_back(mem.dev<uint64_t>((size_t)Kc * V)); }
         r.slot_of = plan->d_slot_of;
     }
     {   // the control tables as one image (CtlTables), uploaded once
@@ -789,9 +777,8 @@ static bool lower(fw_ctx* c, const Schedule& s, Plan* plan, std::string* why) {
         fuse_generic(s, plan);
     }
     if (!alloc_plan(c, plan, !chain, why)) return false;
-    // delay cursors, reverb history cursors + tensor maps, resampler positions and plugin calls change from call to call
     plan->graphable = true;
-    for (auto& st : plan->states) if (st->kind == FW_NODE_DELAY || st->kind == FW_NODE_CONV_REVERB || st->kind == FW_NODE_RESAMPLER || st->kind == FW_NODE_CUSTOM) plan->graphable = false;
+    for (auto& st : plan->states) if (node_kind(st->kind).call_varying) plan->graphable = false;
     for (auto& st : plan->states) if (st->kind == FW_NODE_CONV_REVERB) plan->heavy_stage = true;
     return true;
 }
@@ -951,15 +938,13 @@ int fw_graph_node_info(fw_ctx* c, fw_node_id node, fw_node_info* out) {
     if (out) {
         std::memset(out, 0, sizeof(*out));
         out->num_inputs = r->num_inputs; out->num_outputs = r->num_outputs; out->kind = r->params->kind;
-        node_supported_ports(r->params->kind, &out->num_min_supported_inputs, &out->num_max_supported_inputs, &out->num_min_supported_outputs, &out->num_max_supported_outputs);
-        const char* name = r->id == c->graph->graph_in() ? "graph_in" : r->id == c->graph->graph_out() ? "graph_out" : node_debug_name(r->params->kind);
-        out->updates = r->params->kind == FW_NODE_SAMPLER;  // sampler.rs:193
-        if (r->params->custom) {
-            const fw_audio_node_info& ci = r->params->custom->info;
-            out->num_min_supported_inputs = ci.num_min_supported_inputs; out->num_max_supported_inputs = ci.num_max_supported_inputs;
-            out->num_min_supported_outputs = ci.num_min_supported_outputs; out->num_max_supported_outputs = ci.num_max_supported_outputs;
-            out->updates = ci.updates != 0; name = r->params->custom->debug_name.c_str();
-        }
+        const NodeKind& nk = node_kind(r->params->kind);
+        const fw_audio_node_info& ai = r->params->custom ? r->params->custom->info : nk.info;
+        out->num_min_supported_inputs = ai.num_min_supported_inputs; out->num_max_supported_inputs = ai.num_max_supported_inputs;
+        out->num_min_supported_outputs = ai.num_min_supported_outputs; out->num_max_supported_outputs = ai.num_max_supported_outputs;
+        out->updates = ai.updates != 0;
+        const char* name = r->id == c->graph->graph_in() ? "graph_in" : r->id == c->graph->graph_out() ? "graph_out" :
+                           r->params->custom ? r->params->custom->debug_name.c_str() : nk.name;
         std::strncpy(out->debug_name, name, sizeof(out->debug_name) - 1);
     }
     return 1;
@@ -1367,8 +1352,7 @@ int fw_ctx_update(fw_ctx* c, fw_update_status* out) {  // context.rs:93-148
     c->graph->each_node([&](Id id, NodeRec& r) {
         auto it = c->node_states.find(id.pack());
         if (it == c->node_states.end()) return;
-        const uint32_t k = it->second->kind;
-        if ((k == FW_NODE_BIQUAD || k == FW_NODE_SVF || k == FW_NODE_DELAY || k == FW_NODE_CONV_REVERB) && it->second->channels != r.num_inputs) {
+        if (node_kind(it->second->kind).per_channel_state && it->second->channels != r.num_inputs) {
             c->node_states.erase(it);
             if (std::find(c->graph->nodes_to_activate.begin(), c->graph->nodes_to_activate.end(), id) == c->graph->nodes_to_activate.end()) c->graph->nodes_to_activate.push_back(id);
         }
@@ -1393,7 +1377,7 @@ int fw_ctx_update(fw_ctx* c, fw_update_status* out) {  // context.rs:93-148
                     ds->custom_proc = proc_h;
                 }
             }
-            if ((ds->kind == FW_NODE_SAMPLER || ds->kind == FW_NODE_RESAMPLER) && !c->res) c->res = std::make_shared<ResTable>(c->cfg.device);
+            if (node_kind(ds->kind).reads_resources && !c->res) c->res = std::make_shared<ResTable>(c->cfg.device);
             if (!ds->create()) msg = "device allocation failed: " + g_dev_err;
         }
         if (!msg.empty()) {
@@ -1728,10 +1712,10 @@ static int enqueue_chunk(fw_processor* p, Plan& pl, const float* d_in, float* d_
         for (uint32_t b : sp.clear) { if (!FW_CUDA(launch_fill(pl.d_pool + (size_t)b * V * T, (size_t)V * T, 0.0f, p->stream))) return FW_PROC_DEVICE_ERROR; p->launches++; }
         int rc = FW_PROC_OK;
         switch (sp.kind) {
-            case Plan::Step::SAMPLER: rc = run_sampler(p, pl, ck, *sp.node, pl.smp[sp.sampler_idx].rec, sp.sm0, rows, nb); break;
-            case Plan::Step::TEMPORAL: rc = run_temporal(p, sp.node.get(), sp.delay.get(), rows, nb, T, zf); break;
-            case Plan::Step::REVERB: rc = run_reverb(p, *sp.node, rows, nb, T, zf); break;
-            case Plan::Step::PROG:
+            case STEP_SAMPLER: rc = run_sampler(p, pl, ck, *sp.node, pl.smp[sp.sampler_idx].rec, sp.sm0, rows, nb); break;
+            case STEP_TEMPORAL: rc = run_temporal(p, sp.node.get(), sp.delay.get(), rows, nb, T, zf); break;
+            case STEP_REVERB: rc = run_reverb(p, *sp.node, rows, nb, T, zf); break;
+            case STEP_PROG:
                 if (pl.bus && si + 1 == pl.steps.size()) {
                     ChainArgs xa = chain_args(pl, ck, sp.prog, in, ivs, out, ovs, caller);
                     rc = run_bus_stage(p, pl, xa, pl.c_out, ck, d_out + ck.t0);
@@ -1749,7 +1733,7 @@ static int enqueue_chunk(fw_processor* p, Plan& pl, const float* d_in, float* d_
                     if (!FW_LAUNCH(p, 1, 1, launch_silence_fix(fa, p->stream))) return FW_PROC_DEVICE_ERROR;
                 }
                 break;
-            case Plan::Step::SUM:
+            case STEP_SUM:
                 for (uint32_t c = 0, ports = ni / no; c < no; ++c) {
                     SumArgs sa{};
                     for (uint32_t q = 0; q < ports; ++q) { sa.in[q] = in[q * no + c]; sa.mask_bit[q] = (uint8_t)(q * no + c); }
@@ -1759,7 +1743,7 @@ static int enqueue_chunk(fw_processor* p, Plan& pl, const float* d_in, float* d_
                     if (!FW_LAUNCH(p, 1, 1, launch_sum(sa, p->stream))) return FW_PROC_DEVICE_ERROR;
                 }
                 break;
-            case Plan::Step::RESAMPLER: {
+            case STEP_RESAMPLER: {
                 NodeDeviceState& st = *sp.node;
                 ResamplerArgs ra{};
                 for (uint32_t c = 0; c < no; ++c) ra.out[c] = out[c];
@@ -1770,7 +1754,7 @@ static int enqueue_chunk(fw_processor* p, Plan& pl, const float* d_in, float* d_
                 if (!FW_LAUNCH(p, 3, 2, launch_resampler(ra, st.d_rs_pos, p->stream))) return FW_PROC_DEVICE_ERROR;
                 break;
             }
-            case Plan::Step::CUSTOM: {  // AudioNodeProcessor::process for all voices and blocks at once (fw_node_vtable::process_device)
+            case STEP_CUSTOM: {  // AudioNodeProcessor::process for all voices and blocks at once (fw_node_vtable::process_device)
                 NodeDeviceState& st = *sp.node;
                 const uint32_t nblk = (T + pl.block_frames - 1) / pl.block_frames;
                 uint64_t* masks = pl.d_custom_masks[sp.custom_idx];
