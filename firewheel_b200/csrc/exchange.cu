@@ -18,22 +18,16 @@
 
 #include <cstdint>
 
+#include "device.cuh"
 #include "kernels.cuh"
 #include "plan.hpp"
 
 namespace fw {
 namespace {
 
-__device__ __forceinline__ uint32_t ld_acquire_gpu(const uint32_t* p) {
-    uint32_t v;
-    asm volatile("ld.acquire.gpu.global.u32 %0, [%1];" : "=r"(v) : "l"(p) : "memory");
-    return v;
-}
-__device__ __forceinline__ void st_release_gpu(uint32_t* p, uint32_t v) { asm volatile("st.release.gpu.global.u32 [%0], %1;" ::"l"(p), "r"(v) : "memory"); }
-
 __global__ void __launch_bounds__(32) bus_signal_kernel(uint32_t* word, uint32_t epoch) {
-    asm volatile("griddepcontrol.launch_dependents;" ::: "memory");  // the next call's control kernel follows like any kernel of the chain
-    asm volatile("griddepcontrol.wait;" ::: "memory");               // the rank-local bus is complete
+    pdl_launch_dependents();  // the next call's control kernel follows like any kernel of the chain
+    pdl_wait();               // the rank-local bus is complete
     if (threadIdx.x == 0) { __threadfence(); st_release_gpu(word, epoch); }
 }
 
@@ -50,12 +44,7 @@ __global__ void __launch_bounds__(32) bus_wait_kernel(const uint32_t* word, uint
 }  // namespace
 
 cudaError_t launch_bus_signal(uint32_t* word, uint32_t epoch, cudaStream_t st) {
-    cudaLaunchConfig_t cfg{};
-    cfg.gridDim = dim3(1); cfg.blockDim = dim3(32); cfg.stream = st;
-    cudaLaunchAttribute at[1];
-    at[0].id = cudaLaunchAttributeProgrammaticStreamSerialization; at[0].val.programmaticStreamSerializationAllowed = 1;
-    cfg.attrs = at; cfg.numAttrs = 1;
-    return cudaLaunchKernelEx(&cfg, bus_signal_kernel, word, epoch);
+    return launch_ex(bus_signal_kernel, dim3(1), dim3(32), 0, st, true, word, epoch);
 }
 cudaError_t launch_bus_wait(const uint32_t* word, uint32_t epoch, uint32_t* error, uint32_t error_value, cudaStream_t st) {
     bus_wait_kernel<<<1, 32, 0, st>>>(word, epoch, error, error_value);

@@ -8,7 +8,7 @@
 //   resampler_*_kernel   K-resampler  polyphase windowed-sinc sample player (+ seek / advance helpers)
 //   combine_kernel       K-combine    radix-16 levels of the bus tree over partial buses
 //   (de)interleave, fill, bus_mask    stream boundary and small helpers
-// temporal.cu holds the biquad / SVF / delay kernels, reverb.cu the wgmma FIR GEMM, exchange.cu the stream hand-over of the master-bus exchange.
+// temporal.cu holds the biquad / SVF / delay kernels (biquad_delay_lanes; biquad_delay_generic / svf_generic, the scalar path), reverb.cu the wgmma FIR GEMM, exchange.cu the stream hand-over of the master-bus exchange.
 //
 // Bit-exactness rules (SURVEY.md §7 H2): this TU is compiled with --fmad=false, -ftz=false,
 // -prec-div=true; recurrences additionally spell out __fmul_rn/__fadd_rn. Sum order equals the
@@ -17,9 +17,9 @@
 
 #include <cstdint>
 #include <cstdlib>
-#include <utility>
 
 #include "../../include/fw_b200.h"
+#include "device.cuh"
 #include "kernels.cuh"
 #include "plan.hpp"
 
@@ -35,11 +35,6 @@ namespace fw {
 //   HardClip masks      hard_clip.rs:60-93
 // Only state transitions and gain curves are computed here; no sample data is touched.
 // =============================================================================================
-// Programmatic dependent launch (sm_90+): a kernel launched with the PDL attribute may start while its
-// predecessor in the stream is still running; it must not touch the predecessor's results before pdl_wait().
-__device__ __forceinline__ void pdl_launch_dependents() { asm volatile("griddepcontrol.launch_dependents;" ::: "memory"); }
-__device__ __forceinline__ void pdl_wait() { asm volatile("griddepcontrol.wait;" ::: "memory"); }
-
 struct SmLocal { float input, last; uint32_t status; };
 
 __device__ __forceinline__ uint64_t all_silent_mask(uint32_t n) { return n >= 64 ? ~0ull : ((1ull << n) - 1ull); }
@@ -168,9 +163,8 @@ __global__ void __launch_bounds__(128) control_kernel(const __grid_constant__ Co
     const SmDesc* const smd = reinterpret_cast<const SmDesc*>(tab + tb.o_sm);
     const SamplerCtl* const smp = reinterpret_cast<const SamplerCtl*>(tab + tb.o_smp);
     const RsCtl* const rsc = reinterpret_cast<const RsCtl*>(tab + tb.o_rs);
-    const uint32_t NS = tb.n_smoothers, F = a.block_frames, NSMP = tb.n_samplers, MW = a.rec.n_mode_words;
+    const uint32_t F = a.block_frames, NSMP = tb.n_samplers, MW = a.rec.n_mode_words;
     const uint32_t n_blocks = (a.frames + F - 1) / F;
-    uint16_t* slot_of = const_cast<uint16_t*>(a.rec.slot_of);
     uint64_t* const fl = s_dyn + threadIdx.x;            // word w >= 1: fl[(w - 1) * B]
     uint64_t* const fl0 = fl + (size_t)(W - 1) * B;       // its value at the start of the block
 
@@ -210,9 +204,9 @@ __global__ void __launch_bounds__(128) control_kernel(const __grid_constant__ Co
                         smp_step(q, a.res_tab[q.res - 1].frames, frames, &r, dummy);
                         sc.playhead[v] = q.playhead;  // the only field a replayed block moves
                     }
-                    sc.rec[(size_t)k * V + v] = r;
+                    Records::at_kv(sc.rec, k, v, V) = r;
                 }
-                slot_of[(size_t)k * V + v] = (uint16_t)slot;
+                Records::at_kv(a.rec.slot_of, k, v, V) = (uint16_t)slot;
                 continue;
             }
             steady_mode = false; steady = 0xffffffffu; ++slot;
@@ -224,17 +218,16 @@ __global__ void __launch_bounds__(128) control_kernel(const __grid_constant__ Co
         // Mode words of this record: smoothers are numbered in schedule order, so the walk meets them word by word and each word
         // is stored once, when the walk has moved past it.
         uint32_t mw = 0, mword = 0, mor = 0;
-        uint32_t* const modes = a.rec.modes + (size_t)slot * MW * V + v;
         auto put_mode = [&](int32_t s, uint32_t m) {
             const uint32_t w = (uint32_t)s / kModesPerWord;
-            for (; mw < w; ++mw) { modes[(size_t)mw * V] = mword; mor |= mword; mword = 0; }
+            for (; mw < w; ++mw) { a.rec.mode_word(slot, mw, v, V) = mword; mor |= mword; mword = 0; }
             mword |= m << (2 * ((uint32_t)s % kModesPerWord));
         };
         auto put_val = [&](int32_t s, float cv) {
-            a.rec.vals[((size_t)slot * NS + s) * V + v] = cv;
-            a.rec.st_vals[(size_t)s * V + v] = cv;  // the last value written is the steady record's
+            a.rec.val(slot, s, v, V) = cv;
+            a.rec.st_val(s, v, V) = cv;  // the last value written is the steady record's
         };
-        auto curve_of = [&](int32_t s) { return a.rec.curves + (((size_t)slot * NS + s) * V + v) * F; };
+        auto curve_of = [&](int32_t s) { return a.rec.curve(slot, s, v, V, F); };
         for (uint32_t n = 0; n < tb.n_nodes; ++n) {
             const CtlNode nd = nodes[n];
             uint64_t in_mask = 0;
@@ -247,8 +240,8 @@ __global__ void __launch_bounds__(128) control_kernel(const __grid_constant__ Co
                 if (set) in_mask |= 1ull << i;
             }
             if (nd.mask_slot) {
-                a.rec.sum_masks[((size_t)slot * a.rec.n_sum_masks + (nd.mask_slot - 1)) * V + v] = in_mask;
-                a.rec.st_sum_masks[(size_t)(nd.mask_slot - 1) * V + v] = in_mask;  // the last mask written is the steady record's
+                a.rec.in_mask(slot, nd.mask_slot - 1, v, V) = in_mask;
+                a.rec.st_in_mask(nd.mask_slot - 1, v, V) = in_mask;  // the last mask written is the steady record's
             }
             uint64_t out_mask = 0;  // processor.rs:233 NONE_SILENT
             switch (nd.kind) {
@@ -323,7 +316,7 @@ __global__ void __launch_bounds__(128) control_kernel(const __grid_constant__ Co
                     else if (nd.n_out > sch && !(nd.n_out == 2 && sch == 1))  // :545-559: channels past the sample's are zeroed and flagged
                         out_mask = all_silent_mask(nd.n_out) & ~all_silent_mask(sch);
                     sc.last_play[v] = play ? 1u : 0u;
-                    sc.rec[(size_t)k * V + v] = r;
+                    Records::at_kv(sc.rec, k, v, V) = r;
                     break;
                 }
                 case FW_NODE_RESAMPLER: {  // spec ours: cleared + flagged when not playing / no resource; surplus channels as the sampler's
@@ -361,9 +354,9 @@ __global__ void __launch_bounds__(128) control_kernel(const __grid_constant__ Co
                 else { uint64_t& word = fl[((b >> 6) - 1) * B]; word = set ? (word | bit) : (word & ~bit); }
             }
         }
-        for (; mw < MW; ++mw) { modes[(size_t)mw * V] = mword; mor |= mword; mword = 0; }
+        for (; mw < MW; ++mw) { a.rec.mode_word(slot, mw, v, V) = mword; mor |= mword; mword = 0; }
         last_modes = mor;
-        if (slot_of) slot_of[(size_t)k * V + v] = (uint16_t)slot;
+        if (a.rec.slot_of) Records::at_kv(a.rec.slot_of, k, v, V) = (uint16_t)slot;
         bool same = f0 == f0_start;
         for (uint32_t w = 1; w < W; ++w) same = same && fl0[(w - 1) * B] == fl[(w - 1) * B];
         if (!changed && same) {  // nothing moved: later blocks replay this record
@@ -406,61 +399,44 @@ template <> struct VecT<1> {
     static __device__ __forceinline__ void store(float* p, const float (&x)[1]) { __stcs(p, x[0]); }
 };
 
-// record slot of block k of voice v (see Records::slot_of)
-__device__ __forceinline__ uint32_t rec_slot(const Records& r, uint32_t v, uint32_t k, uint32_t V) {
-    if (r.slot_of != nullptr) return r.slot_of[(size_t)k * V + v];
-    return min(k, r.steady_k[v]);
-}
-
-// mode of smoother s in a record: modes points at word 0 of the (slot, voice), words are V apart
-__device__ __forceinline__ uint32_t rec_mode(const uint32_t* modes, uint32_t V, uint32_t s) {
-    return (modes[(size_t)(s / kModesPerWord) * V] >> (2 * (s % kModesPerWord))) & 3u;
-}
-
-struct RecView {  // per-voice record access, either from the CTA's smem stage or straight from global
-    uint32_t kk;
-    const uint32_t* modes;  // word w of the record: modes[w * V]
-    const float* vals;  // vals[s * stride]
-    uint32_t stride;
-};
-
+// the program on one voice's tile, reading record slot kk
 template <int VEC>
-__device__ __forceinline__ void apply_chain(const ChainArgs& a, const RecView& r, uint32_t v, uint32_t t_in_block, float (&x)[2][VEC]) {
-    const uint32_t NS = a.rec.n_smoothers, V = a.num_voices, F = a.block_frames;
+__device__ __forceinline__ void apply_chain(const ChainArgs& a, uint32_t kk, uint32_t v, uint32_t t_in_block, float (&x)[2][VEC]) {
+    const uint32_t V = a.num_voices, F = a.block_frames;
 #pragma unroll 1
     for (uint32_t o = 0; o < a.prog.n_ops; ++o) {
         const ChainOp op = a.prog.ops[o];
         switch (op.kind) {
             case OP_GAIN: {  // volume.rs:116-143: out = in * gain[i] (both channels share the curve)
-                const uint32_t m = rec_mode(r.modes, V, (uint32_t)op.sm0);
+                const uint32_t m = a.rec.mode(kk, (uint32_t)op.sm0, v, V);
                 if (m == REC_CLEAR) {
 #pragma unroll
                     for (int i = 0; i < VEC; ++i) { x[0][i] = 0.0f; x[1][i] = 0.0f; }
                 } else if (m == REC_CONST) {
-                    const float g = r.vals[op.sm0 * r.stride];
+                    const float g = a.rec.val(kk, op.sm0, v, V);
 #pragma unroll
                     for (int i = 0; i < VEC; ++i) { x[0][i] = __fmul_rn(x[0][i], g); x[1][i] = __fmul_rn(x[1][i], g); }
                 } else {
                     float g[VEC];
-                    VecT<VEC>::load_ca(a.rec.curves + ((size_t)(r.kk * NS + op.sm0) * V + v) * F + t_in_block, g);
+                    VecT<VEC>::load_ca(a.rec.curve(kk, op.sm0, v, V, F) + t_in_block, g);
 #pragma unroll
                     for (int i = 0; i < VEC; ++i) { x[0][i] = __fmul_rn(x[0][i], g[i]); x[1][i] = __fmul_rn(x[1][i], g[i]); }
                 }
                 break;
             }
             case OP_PAN: {
-                const uint32_t m0 = rec_mode(r.modes, V, (uint32_t)op.sm0), m1 = rec_mode(r.modes, V, (uint32_t)op.sm1);
+                const uint32_t m0 = a.rec.mode(kk, (uint32_t)op.sm0, v, V), m1 = a.rec.mode(kk, (uint32_t)op.sm1, v, V);
                 if (m0 == REC_CLEAR) {
 #pragma unroll
                     for (int i = 0; i < VEC; ++i) { x[0][i] = 0.0f; x[1][i] = 0.0f; }
                 } else {
                     float gl[VEC], gr[VEC];
-                    if (m0 == REC_CURVE) VecT<VEC>::load_ca(a.rec.curves + ((size_t)(r.kk * NS + op.sm0) * V + v) * F + t_in_block, gl);
-                    else { const float g = r.vals[op.sm0 * r.stride];
+                    if (m0 == REC_CURVE) VecT<VEC>::load_ca(a.rec.curve(kk, op.sm0, v, V, F) + t_in_block, gl);
+                    else { const float g = a.rec.val(kk, op.sm0, v, V);
 #pragma unroll
                         for (int i = 0; i < VEC; ++i) gl[i] = g; }
-                    if (m1 == REC_CURVE) VecT<VEC>::load_ca(a.rec.curves + ((size_t)(r.kk * NS + op.sm1) * V + v) * F + t_in_block, gr);
-                    else { const float g = r.vals[op.sm1 * r.stride];
+                    if (m1 == REC_CURVE) VecT<VEC>::load_ca(a.rec.curve(kk, op.sm1, v, V, F) + t_in_block, gr);
+                    else { const float g = a.rec.val(kk, op.sm1, v, V);
 #pragma unroll
                         for (int i = 0; i < VEC; ++i) gr[i] = g; }
 #pragma unroll
@@ -494,7 +470,7 @@ __global__ void __launch_bounds__(kWarps * 32, kMinBlocks) chain_kernel(ChainArg
     static_assert(kVPW * kWarps == kVPC, "a CTA owns 64 voices");
     pdl_launch_dependents();
     const uint32_t lane = threadIdx.x & 31u, warp = threadIdx.x >> 5;
-    const uint32_t T = a.frames, V = a.num_voices, F = a.block_frames, NS = a.rec.n_smoothers, MW = a.rec.n_mode_words;
+    const uint32_t T = a.frames, V = a.num_voices, F = a.block_frames;
     // Bus variant: CTA slice z sums channels 2z and 2z + 1 of a C-channel bus (C = prog.c_out, up to kMaxBusChannels), an odd last
     // channel alone; the channels are independent trees, so a bus over C channels is ceil(C / 2) stereo reductions on grid.z.
     const uint32_t zc = BUS ? 2u * blockIdx.z : 0u;
@@ -552,7 +528,7 @@ __global__ void __launch_bounds__(kWarps * 32, kMinBlocks) chain_kernel(ChainArg
         if (lane < kVPW && v0 + lane < V) special = (kb < a.rec.steady_k[v0 + lane]) || (a.rec.st_modes[v0 + lane] != 0u);
         for (uint32_t i = lane; i < a.prog.n_sm * kVPW; i += 32u) {
             const uint32_t s = i / kVPW, j = i % kVPW;
-            s_wv[warp][s][j] = (v0 + j < V) ? a.rec.st_vals[(size_t)a.prog.sm[s] * V + v0 + j] : 0.0f;
+            s_wv[warp][s][j] = (v0 + j < V) ? a.rec.st_val(a.prog.sm[s], v0 + j, V) : 0.0f;
         }
         warp_fast = !__any_sync(0xffffffffu, special);
         __syncwarp();
@@ -607,12 +583,7 @@ __global__ void __launch_bounds__(kWarps * 32, kMinBlocks) chain_kernel(ChainArg
 #pragma unroll 1
         for (int j = 0; j < kVPW; ++j) {  // xs is indexed dynamically on purpose: it lives in local memory
             const uint32_t v = v0 + j;
-            if (v < V && t_ok) {
-                RecView r;
-                r.kk = rec_slot(a.rec, v, k, V); r.modes = a.rec.modes + (size_t)r.kk * MW * V + v;
-                r.vals = a.rec.vals + (size_t)r.kk * NS * V + v; r.stride = V;
-                apply_chain<VEC>(a, r, v, t_in_block, xs[j]);
-            }
+            if (v < V && t_ok) apply_chain<VEC>(a, a.rec.slot(k, v, V), v, t_in_block, xs[j]);
         }
 #pragma unroll
         for (int j = 0; j < kVPW; ++j)
@@ -692,10 +663,7 @@ __global__ void __launch_bounds__(128) sum_kernel(const __grid_constant__ SumArg
     if (t >= T) return;
     const size_t off = (size_t)v * T + t;
     uint64_t mask = 0;
-    if (a.mask_slot >= 0) {
-        const uint32_t k = t / a.block_frames, sk = a.rec.steady_k[v];
-        mask = k >= sk ? a.rec.st_sum_masks[(size_t)a.mask_slot * V + v] : a.rec.sum_masks[((size_t)rec_slot(a.rec, v, k, V) * a.rec.n_sum_masks + a.mask_slot) * V + v];
-    }
+    if (a.mask_slot >= 0) mask = a.rec.block_in_mask(t / a.block_frames, a.mask_slot, v, V);
     float acc[VEC];
     if (a.mask_slot >= 0 && (mask & a.all_mask) == a.all_mask) {
 #pragma unroll
@@ -724,8 +692,7 @@ __global__ void __launch_bounds__(128) silence_fix_kernel(const __grid_constant_
     pdl_wait();
     const uint32_t t = (blockIdx.y * blockDim.x + threadIdx.x) * VEC, v = blockIdx.x, T = a.frames, V = a.num_voices;  // voices on grid.x (no 65535 cap)
     if (t >= T) return;
-    const uint32_t k = t / a.block_frames, sk = a.rec.steady_k[v];
-    const uint64_t mask = k >= sk ? a.rec.st_sum_masks[(size_t)a.mask_slot * V + v] : a.rec.sum_masks[((size_t)rec_slot(a.rec, v, k, V) * a.rec.n_sum_masks + a.mask_slot) * V + v];
+    const uint64_t mask = a.rec.block_in_mask(t / a.block_frames, a.mask_slot, v, V);
     if ((mask & a.test) != a.test) return;
     float z[VEC];
 #pragma unroll
@@ -739,8 +706,7 @@ __global__ void __launch_bounds__(128) expand_masks_kernel(Records rec, uint32_t
     pdl_wait();
     const uint32_t v = blockIdx.x * blockDim.x + threadIdx.x, k = blockIdx.y;
     if (v >= V || k >= n_blocks) return;
-    out[(size_t)k * V + v] = k >= rec.steady_k[v] ? rec.st_sum_masks[(size_t)mask_slot * V + v]
-                                                  : rec.sum_masks[((size_t)rec_slot(rec, v, k, V) * rec.n_sum_masks + mask_slot) * V + v];
+    Records::at_kv(out, k, v, V) = rec.block_in_mask(k, mask_slot, v, V);
 }
 
 // K-sampler: SamplerNode data plane (sampler.rs:445-559 + sample_resource.rs:337-456). One thread = VEC frames of one
@@ -764,7 +730,7 @@ __global__ void __launch_bounds__(128) sampler_kernel(const __grid_constant__ Sa
     const uint32_t t = (blockIdx.y * blockDim.x + threadIdx.x) * VEC, v = blockIdx.x, c = blockIdx.z, T = a.frames, V = a.num_voices, F = a.block_frames;
     if (t >= T) return;
     const uint32_t k = t / F, f0 = t - k * F;
-    const SmpRec r = a.srec[(size_t)k * V + v];
+    const SmpRec r = Records::at_kv(a.srec, k, v, V);
     float y[VEC];
 #pragma unroll
     for (int i = 0; i < VEC; ++i) y[i] = 0.0f;
@@ -777,14 +743,15 @@ __global__ void __launch_bounds__(128) sampler_kernel(const __grid_constant__ Sa
         if (a.n_out == 2 && d.channels == 1) src_ch = 0;              // :546-551 mono sample, stereo node: duplicate
         else { VecT<VEC>::store(dst, y); return; }                    // :552-558 zeroed (and flagged by the control kernel)
     }
-    const uint32_t kk = rec_slot(a.rec, v, k, V), NS = a.rec.n_smoothers;
-    const uint32_t m = rec_mode(a.rec.modes + (size_t)kk * a.rec.n_mode_words * V + v, V, (uint32_t)a.sm);
+    const uint32_t kk = a.rec.slot(k, v, V);
+    const uint32_t m = a.rec.mode(kk, (uint32_t)a.sm, v, V);
     float g[VEC];
     if (m == REC_CURVE) {
+        const float* curve = a.rec.curve(kk, a.sm, v, V, F) + f0;
 #pragma unroll
-        for (int i = 0; i < VEC; ++i) g[i] = a.rec.curves[((size_t)(kk * NS + a.sm) * V + v) * F + f0 + i];
+        for (int i = 0; i < VEC; ++i) g[i] = curve[i];
     } else {
-        const float gc = a.rec.vals[(size_t)(kk * NS + a.sm) * V + v];
+        const float gc = a.rec.val(kk, a.sm, v, V);
 #pragma unroll
         for (int i = 0; i < VEC; ++i) g[i] = gc;
     }
@@ -866,7 +833,7 @@ __global__ void __launch_bounds__(128) combine_kernel(const float* __restrict__ 
         if (threadIdx.x == 0 && atomicAdd(done_counter, 1u) == gridDim.x * gridDim.y * gridDim.z - 1u) {
             *done_counter = 0u;
             __threadfence();
-            asm volatile("st.release.gpu.global.u32 [%0], %1;" ::"l"(done_word), "r"(done_epoch) : "memory");
+            st_release_gpu(done_word, done_epoch);
         }
     }
 }
@@ -933,21 +900,13 @@ __global__ void bus_mask_kernel(const uint64_t* __restrict__ gout_mask, uint32_t
 static inline unsigned grid_for(size_t n) { size_t b = (n + 255) / 256; return (unsigned)(b < 132u * 16u ? b : 132u * 16u); }
 #define FW_LAUNCH_CHECK() do { cudaError_t e_ = cudaGetLastError(); if (e_ != cudaSuccess) return e_; } while (0)
 
-// All three per-call kernels are launched with programmatic stream serialization: each begins with
-// griddepcontrol.launch_dependents and reads its predecessor's results only after griddepcontrol.wait.
-template <class... KArgs, class... Args>
-static cudaError_t launch_pdl_smem(void (*kernel)(KArgs...), dim3 grid, dim3 block, size_t smem, cudaStream_t st, Args&&... args) {
-    cudaLaunchConfig_t cfg{};
-    cfg.gridDim = grid; cfg.blockDim = block; cfg.dynamicSmemBytes = smem; cfg.stream = st;
-    cudaLaunchAttribute attr[1];
-    attr[0].id = cudaLaunchAttributeProgrammaticStreamSerialization;
-    attr[0].val.programmaticStreamSerializationAllowed = 1;
-    cfg.attrs = attr; cfg.numAttrs = 1;
-    return cudaLaunchKernelEx(&cfg, kernel, std::forward<Args>(args)...);
-}
-template <class... KArgs, class... Args>
-static cudaError_t launch_pdl(void (*kernel)(KArgs...), dim3 grid, dim3 block, cudaStream_t st, Args&&... args) {
-    return launch_pdl_smem(kernel, grid, block, 0, st, std::forward<Args>(args)...);
+// The per-call kernels here are launched with programmatic stream serialization (pdl = true): each begins with
+// pdl_launch_dependents() and reads its predecessor's results only after pdl_wait().
+
+// 4-wide vectors when both frame counts are multiples of 4 and `addr_bits`, the OR of every address and byte stride the kernel
+// steps through, is a multiple of 16
+static bool vec4_ok(uint32_t frames, uint32_t block_frames, uintptr_t addr_bits) {
+    return frames % 4 == 0 && block_frames % 4 == 0 && addr_bits % 16 == 0;
 }
 
 // Threads per CTA of the control kernel: 128 while the shared-memory flags of a voice (two copies of words 1 .. n_flag_words - 1) fit in
@@ -974,14 +933,14 @@ cudaError_t launch_control(ControlArgs a, cudaStream_t st) {
         const cudaError_t e = cudaFuncSetAttribute(control_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
         if (e != cudaSuccess) return e;
     }
-    return launch_pdl_smem(control_kernel, dim3((a.num_voices + threads - 1) / threads), dim3(threads), smem, st, a);
+    return launch_ex(control_kernel, dim3((a.num_voices + threads - 1) / threads), dim3(threads), smem, st, true, a);
 }
 
 template <int VEC, int CIN, int VPW, int WARPS, int MINB>
 static cudaError_t launch_chain_v(const ChainArgs& a, bool bus, cudaStream_t st) {
     dim3 grid((a.frames + 32 * VEC - 1) / (32 * VEC), (a.num_voices + kVPC - 1) / kVPC, bus ? (a.prog.c_out + 1) / 2 : 1);
-    if (bus) return launch_pdl(chain_kernel<VEC, CIN, true, VPW, WARPS, MINB>, grid, dim3(WARPS * 32), st, a);
-    return launch_pdl(chain_kernel<VEC, CIN, false, VPW, WARPS, MINB>, grid, dim3(WARPS * 32), st, a);
+    if (bus) return launch_ex(chain_kernel<VEC, CIN, true, VPW, WARPS, MINB>, grid, dim3(WARPS * 32), 0, st, true, a);
+    return launch_ex(chain_kernel<VEC, CIN, false, VPW, WARPS, MINB>, grid, dim3(WARPS * 32), 0, st, true, a);
 }
 template <int VEC, int CIN>
 static cudaError_t launch_chain_t(const ChainArgs& a, bool bus, cudaStream_t st) {
@@ -992,7 +951,7 @@ cudaError_t launch_chain(const ChainArgs& a, bool bus, cudaStream_t st) {
     uintptr_t al = reinterpret_cast<uintptr_t>(a.out_ch[0]) | reinterpret_cast<uintptr_t>(a.out_ch[1]) | reinterpret_cast<uintptr_t>(a.out) |
                    (uintptr_t)((a.in_vstride | a.out_vstride | a.bus_pitch) * 4);
     for (const float* q : a.in_ch) al |= reinterpret_cast<uintptr_t>(q);
-    const bool vec4 = (a.frames % 4 == 0) && (a.block_frames % 4 == 0) && (al % 16 == 0);
+    const bool vec4 = vec4_ok(a.frames, a.block_frames, al);
     if (a.prog.c_in >= 2) return vec4 ? launch_chain_t<4, 2>(a, bus, st) : launch_chain_t<1, 2>(a, bus, st);
     return vec4 ? launch_chain_t<4, 1>(a, bus, st) : launch_chain_t<1, 1>(a, bus, st);
 }
@@ -1001,25 +960,24 @@ uint32_t chain_voice_groups(uint32_t num_voices) { return (num_voices + kVPC - 1
 cudaError_t launch_combine(const float* pin, float* pout, uint32_t n_in, uint32_t rows, uint32_t T, cudaStream_t st, uint32_t out_pitch,
                            uint32_t* done_word, uint32_t* done_counter, uint32_t done_epoch) {
     if (out_pitch == 0) out_pitch = T;
-    const bool vec4 = (T % 4 == 0) && (out_pitch % 4 == 0) && ((reinterpret_cast<uintptr_t>(pin) | reinterpret_cast<uintptr_t>(pout)) % 16 == 0);
+    // a row of the bus is one block
+    const bool vec4 = vec4_ok(T, T, reinterpret_cast<uintptr_t>(pin) | reinterpret_cast<uintptr_t>(pout) | (uintptr_t)out_pitch * 4);
     const uint32_t n_out = (n_in + 15) / 16;
-    if (vec4) return launch_pdl(combine_kernel<4>, dim3((T / 4 + 127) / 128, rows, n_out), dim3(128), st, pin, pout, n_in, rows, T, out_pitch, done_word, done_counter, done_epoch);
-    return launch_pdl(combine_kernel<1>, dim3((T + 127) / 128, rows, n_out), dim3(128), st, pin, pout, n_in, rows, T, out_pitch, done_word, done_counter, done_epoch);
+    if (vec4) return launch_ex(combine_kernel<4>, dim3((T / 4 + 127) / 128, rows, n_out), dim3(128), 0, st, true, pin, pout, n_in, rows, T, out_pitch, done_word, done_counter, done_epoch);
+    return launch_ex(combine_kernel<1>, dim3((T + 127) / 128, rows, n_out), dim3(128), 0, st, true, pin, pout, n_in, rows, T, out_pitch, done_word, done_counter, done_epoch);
 }
 cudaError_t launch_sum(const SumArgs& a, cudaStream_t st) {
     uintptr_t al = reinterpret_cast<uintptr_t>(a.out);
     for (uint32_t p = 0; p < a.n_ports; ++p) al |= reinterpret_cast<uintptr_t>(a.in[p]);
-    const bool vec4 = (a.frames % 4 == 0) && (a.block_frames % 4 == 0) && (al % 16 == 0);
-    if (vec4) return launch_pdl(sum_kernel<4>, dim3(a.num_voices, (a.frames / 4 + 127) / 128), dim3(128), st, a);
-    return launch_pdl(sum_kernel<1>, dim3(a.num_voices, (a.frames + 127) / 128), dim3(128), st, a);
+    if (vec4_ok(a.frames, a.block_frames, al)) return launch_ex(sum_kernel<4>, dim3(a.num_voices, (a.frames / 4 + 127) / 128), dim3(128), 0, st, true, a);
+    return launch_ex(sum_kernel<1>, dim3(a.num_voices, (a.frames + 127) / 128), dim3(128), 0, st, true, a);
 }
 cudaError_t launch_sampler(const SamplerArgs& a, cudaStream_t st) {
     if (a.n_out == 0 || a.num_voices == 0 || a.frames == 0) return cudaSuccess;
-    uintptr_t al = 0;
+    uintptr_t al = (uintptr_t)(a.out_vstride * 4);
     for (uint32_t c = 0; c < a.n_out; ++c) al |= reinterpret_cast<uintptr_t>(a.out[c]);
-    const bool vec4 = (a.frames % 4 == 0) && (a.block_frames % 4 == 0) && (al % 16 == 0) && (a.out_vstride % 4 == 0);
-    if (vec4) return launch_pdl(sampler_kernel<4>, dim3(a.num_voices, (a.frames / 4 + 127) / 128, a.n_out), dim3(128), st, a);
-    return launch_pdl(sampler_kernel<1>, dim3(a.num_voices, (a.frames + 127) / 128, a.n_out), dim3(128), st, a);
+    if (vec4_ok(a.frames, a.block_frames, al)) return launch_ex(sampler_kernel<4>, dim3(a.num_voices, (a.frames / 4 + 127) / 128, a.n_out), dim3(128), 0, st, true, a);
+    return launch_ex(sampler_kernel<1>, dim3(a.num_voices, (a.frames + 127) / 128, a.n_out), dim3(128), 0, st, true, a);
 }
 cudaError_t launch_resampler(const ResamplerArgs& a, uint64_t* pos, cudaStream_t st) {
     if (a.n_out && a.num_voices && a.frames) {
@@ -1029,17 +987,16 @@ cudaError_t launch_resampler(const ResamplerArgs& a, uint64_t* pos, cudaStream_t
     return cudaGetLastError();
 }
 cudaError_t launch_silence_fix(const SilenceFixArgs& a, cudaStream_t st) {
-    const bool vec4 = (a.frames % 4 == 0) && (a.block_frames % 4 == 0) && (reinterpret_cast<uintptr_t>(a.out) % 16 == 0);
-    if (vec4) return launch_pdl(silence_fix_kernel<4>, dim3(a.num_voices, (a.frames / 4 + 127) / 128), dim3(128), st, a);
-    return launch_pdl(silence_fix_kernel<1>, dim3(a.num_voices, (a.frames + 127) / 128), dim3(128), st, a);
+    if (vec4_ok(a.frames, a.block_frames, reinterpret_cast<uintptr_t>(a.out))) return launch_ex(silence_fix_kernel<4>, dim3(a.num_voices, (a.frames / 4 + 127) / 128), dim3(128), 0, st, true, a);
+    return launch_ex(silence_fix_kernel<1>, dim3(a.num_voices, (a.frames + 127) / 128), dim3(128), 0, st, true, a);
 }
 cudaError_t launch_expand_masks(const Records& rec, uint32_t mask_slot, uint32_t V, uint32_t n_blocks, uint64_t* out, cudaStream_t st) {
     if (V == 0 || n_blocks == 0) return cudaSuccess;
-    return launch_pdl(expand_masks_kernel, dim3((V + 127) / 128, n_blocks), dim3(128), st, rec, mask_slot, V, n_blocks, out);
+    return launch_ex(expand_masks_kernel, dim3((V + 127) / 128, n_blocks), dim3(128), 0, st, true, rec, mask_slot, V, n_blocks, out);
 }
 cudaError_t launch_poke(const PokeArgs& a, cudaStream_t st) {
     if (a.n == 0) return cudaSuccess;
-    return launch_pdl(poke_kernel, dim3(1), dim3(128), st, a);
+    return launch_ex(poke_kernel, dim3(1), dim3(128), 0, st, true, a);
 }
 cudaError_t launch_deinterleave(const float* inter, float* planar, uint32_t V, uint32_t C, uint32_t T, cudaStream_t st) {
     const size_t n = (size_t)V * C * T; if (n == 0) return cudaSuccess;

@@ -30,7 +30,6 @@ cudaError_t launch_bus_signal(uint32_t* word, uint32_t epoch, cudaStream_t st);
 cudaError_t launch_bus_wait(const uint32_t* word, uint32_t epoch, uint32_t* error, uint32_t error_value, cudaStream_t st);
 cudaError_t launch_poke(const PokeArgs& a, cudaStream_t st);
 cudaError_t launch_temporal(const TemporalArgs& a, cudaStream_t st);
-bool temporal_fast_path(const TemporalArgs& a);
 uint32_t reverb_kpad(uint32_t L);
 uint32_t reverb_hist(uint32_t L);
 uint32_t reverb_grid_max();   // CTAs of the persistent GEMM grid (= SMs)

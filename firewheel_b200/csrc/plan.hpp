@@ -31,7 +31,7 @@ struct CtlNode {
     uint8_t kind, n_in, n_out, pad;
     uint32_t in_off, out_off;   // into CtlTables::in_port / out_port
     int32_t sm0, sm1;           // smoother indices (-1: none); SamplerNode / ResamplerNode: sm1 = index into CtlTables::smp / rs; custom node: sm0 = fw_out_silence_rule
-    uint32_t mask_slot;         // 1 + index into Records::sum_masks, 0 = none
+    uint32_t mask_slot;         // 1 + mask slot of Records::in_masks, 0 = none
 };
 // One smoother: its per-voice state (SoA over voices, owned by the node's device state) and its target parameter
 struct SmDesc { float* input; float* last; uint32_t* status; const float* target; };
@@ -73,24 +73,63 @@ struct CtlTables {
 constexpr uint32_t kCtlParamImage = 2048;  // a table image up to this size also travels in the control kernel's parameters
 constexpr uint32_t kPortClear = 0x80000000u;
 
-// Per-call record buffers written by the control kernel, read by the data kernels.
+// Per-call record buffers written by the control kernel, read by the data kernels. k: record slot (kt_max of them), V voices.
 //   modes[k][w][v]       2 bits per smoother: smoother s in word w = s / 16, bits 2 (s % 16) (n_mode_words = max(1, ceil(NS / 16)))
 //   vals[k][s][v]        constant value of smoother s in block k (REC_CONST)
 //   curves[k][s][v][F]   gain curve (REC_CURVE)
+//   in_masks[k][m][v]    input silence mask of the node with mask slot m (CtlNode::mask_slot - 1): SumNodes, the silence fix, custom nodes
 //   steady_k[v]          blocks >= steady_k[v] reuse the record of block steady_k[v]
 //   st_modes[v]          OR of the steady record's mode words: 0 iff every smoother is REC_CONST there (the chain kernel's fast path)
 //   st_vals[s][v]        the steady record's constant values, flattened so the data kernels reach them with one independent load
+//   st_in_masks[m][v]    the steady record's input masks
+// Every index into these buffers, into slot_of and into the samplers' SmpRec arrays is one of the accessors below. Indices are
+// widened to 64 bits before they are multiplied.
 struct Records {
     uint32_t* modes; float* vals; float* curves; uint32_t* steady_k; uint64_t* gout_mask; uint32_t* error;
     uint32_t* st_modes; float* st_vals;
-    uint64_t* sum_masks; uint64_t* st_sum_masks;  // [k][slot][v] and the steady record [slot][v]
-    uint32_t n_sum_masks, n_mode_words;
+    uint64_t* in_masks; uint64_t* st_in_masks;
+    uint32_t n_mask_slots, n_mode_words;
     uint32_t kt_max, n_smoothers;
     // Graphs with SamplerNodes: a sample that ends mid-call starts a new transient, so "record of block k" is no longer
     // min(k, steady_k): slot_of[k][v] names the record slot explicitly (null for graphs without samplers). steady_k[v] is
     // then the first block of the FINAL steady phase, and st_modes / st_vals its record, so the chain kernel's fast path
     // still applies.
-    const uint16_t* slot_of;
+    uint16_t* slot_of;
+
+    // [block][voice] arrays: slot_of, the samplers' SmpRec records, the custom nodes' dense masks
+    template <class T> __host__ __device__ static T& at_kv(T* p, uint32_t k, uint32_t v, uint32_t V) { return p[(size_t)k * V + v]; }
+    // record slot of block k of voice v
+    __host__ __device__ uint32_t slot(uint32_t k, uint32_t v, uint32_t V) const {
+        if (slot_of != nullptr) return at_kv(slot_of, k, v, V);
+        return min(k, steady_k[v]);
+    }
+    // word w of the mode bits of record slot kk, and the mode of smoother s there
+    __host__ __device__ uint32_t& mode_word(uint32_t kk, uint32_t w, uint32_t v, uint32_t V) const {
+        return (modes + (size_t)kk * n_mode_words * V + v)[(size_t)w * V];
+    }
+    __host__ __device__ uint32_t mode(uint32_t kk, uint32_t s, uint32_t v, uint32_t V) const {
+        return (mode_word(kk, s / kModesPerWord, v, V) >> (2 * (s % kModesPerWord))) & 3u;
+    }
+    __host__ __device__ float& val(uint32_t kk, int32_t s, uint32_t v, uint32_t V) const { return vals[((size_t)kk * n_smoothers + s) * V + v]; }
+    __host__ __device__ float& st_val(int32_t s, uint32_t v, uint32_t V) const { return st_vals[(size_t)s * V + v]; }
+    __host__ __device__ float* curve(uint32_t kk, int32_t s, uint32_t v, uint32_t V, uint32_t F) const {
+        return curves + (((size_t)kk * n_smoothers + s) * V + v) * F;
+    }
+    __host__ __device__ uint64_t& in_mask(uint32_t kk, uint32_t m, uint32_t v, uint32_t V) const { return in_masks[((size_t)kk * n_mask_slots + m) * V + v]; }
+    __host__ __device__ uint64_t& st_in_mask(uint32_t m, uint32_t v, uint32_t V) const { return st_in_masks[(size_t)m * V + v]; }
+    // input mask of mask slot m in block k: the steady record's from steady_k on
+    __host__ __device__ uint64_t block_in_mask(uint32_t k, uint32_t m, uint32_t v, uint32_t V) const {
+        return k >= steady_k[v] ? st_in_mask(m, v, V) : in_mask(slot(k, v, V), m, v, V);
+    }
+
+    // element counts of the buffers for V voices and F frames per block (buffers indexed by smoother or mask slot get at least one row)
+    size_t modes_count(uint32_t V) const { return (size_t)kt_max * n_mode_words * V; }
+    size_t vals_count(uint32_t V) const { return (size_t)kt_max * st_vals_count(V); }
+    size_t curves_count(uint32_t V, uint32_t F) const { return (size_t)kt_max * n_smoothers * V * F; }
+    size_t st_vals_count(uint32_t V) const { return (size_t)(n_smoothers ? n_smoothers : 1) * V; }
+    size_t in_masks_count(uint32_t V) const { return (size_t)kt_max * st_in_masks_count(V); }
+    size_t st_in_masks_count(uint32_t V) const { return (size_t)(n_mask_slots ? n_mask_slots : 1) * V; }
+    static size_t kv_count(uint32_t K, uint32_t V) { return (size_t)K * V; }
 };
 
 // SamplerNode data plane: out[c] + v * out_vstride is channel c of voice v ([T] floats).
@@ -165,7 +204,7 @@ struct SumArgs {
     const float* in[64]; float* out;   // rows [V][T]
     uint8_t mask_bit[64];              // input index (port * n_out + ch) of in[p] inside the node's silence mask
     uint32_t n_ports, num_voices, frames, block_frames;
-    int32_t mask_slot;                 // index into Records::sum_masks
+    int32_t mask_slot;                 // mask slot of Records::in_masks
     uint32_t skip_silent;              // ports >= 5: silent ports are skipped (sum.rs:118-131)
     uint64_t all_mask;                 // all node inputs: every bit set -> outputs cleared (sum.rs:52-56)
     Records rec;

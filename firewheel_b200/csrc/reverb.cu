@@ -26,8 +26,8 @@
 #include <cstdio>
 #include <cstdlib>
 #include <string>
-#include <utility>
 
+#include "device.cuh"
 #include "kernels.cuh"
 #include "plan.hpp"
 #include "wgmma.cuh"
@@ -84,8 +84,8 @@ __global__ void reverb_build_toeplitz(const float* __restrict__ ir, __nv_bfloat1
 // xh[c*V + v][cursor + t] = bf16(in[v][c][t]) for t < T: appends the call's block behind the history (8 samples per thread)
 __global__ void reverb_prepare(const float* __restrict__ in, __nv_bfloat16* __restrict__ xh, uint32_t V, uint32_t C, uint32_t T, uint32_t in_pitch, uint32_t cursor,
                                uint32_t pitch, uint32_t zero_first, uint32_t chan_base) {
-    asm volatile("griddepcontrol.launch_dependents;" ::: "memory");  // the GEMM's set-up (barriers, tensor maps) overlaps this kernel
-    asm volatile("griddepcontrol.wait;" ::: "memory");
+    pdl_launch_dependents();  // the GEMM's set-up (barriers, tensor maps) overlaps this kernel
+    pdl_wait();
     const uint32_t row = blockIdx.x;  // c * V + v (rows on grid.x: no 65535 cap)
     const uint32_t c = row / V, v = row % V;
     __nv_bfloat16* dst = xh + ((size_t)chan_base * V + row) * pitch + cursor;
@@ -127,8 +127,6 @@ __device__ __forceinline__ RvSeg rv_seg(const ReverbGemmArgs& a, uint32_t P, uin
     const uint32_t j = P / a.tail_split, sl = P % a.tail_split;
     return RvSeg{a.full_tiles + j, (uint32_t)((uint64_t)sl * a.num_kb / a.tail_split), (uint32_t)((uint64_t)(sl + 1) * a.num_kb / a.tail_split)};
 }
-__device__ __forceinline__ uint32_t ld_acquire_u32(const uint32_t* p) { uint32_t v; asm volatile("ld.acquire.gpu.global.u32 %0, [%1];" : "=r"(v) : "l"(p) : "memory"); return v; }
-__device__ __forceinline__ void st_release_u32(uint32_t* p, uint32_t v) { asm volatile("st.release.gpu.global.u32 [%0], %1;" ::"l"(p), "r"(v) : "memory"); }
 
 __device__ __forceinline__ void mbar_arrive(uint64_t* bar) { asm volatile("mbarrier.arrive.shared::cta.b64 _, [%0];" ::"r"(smem_u32(bar)) : "memory"); }
 // keeps the accumulators in their registers across the asynchronous MMAs (the compiler must not move or copy them)
@@ -153,7 +151,7 @@ __global__ void __launch_bounds__(RV_THREADS, 1) reverb_gemm_kernel(const __grid
     uint64_t* full_bar = reinterpret_cast<uint64_t*>(smem + RV_STAGES * (RV_A_BYTES + RV_B_BYTES));
     uint64_t* empty_bar = full_bar + RV_STAGES;
 
-    asm volatile("griddepcontrol.launch_dependents;" ::: "memory");  // the next kernel's launch latency hides behind this one; it waits for our results itself
+    pdl_launch_dependents();  // the next kernel's launch latency hides behind this one; it waits for our results itself
     const uint32_t warp = threadIdx.x >> 5, lane = threadIdx.x & 31u;
     const uint32_t P = blockIdx.x, NP = gridDim.x, num_kb = a.num_kb;
 
@@ -171,7 +169,7 @@ __global__ void __launch_bounds__(RV_THREADS, 1) reverb_gemm_kernel(const __grid
 
     if (warp == 0) {
         // ===== TMA producer =====
-        asm volatile("griddepcontrol.wait;" ::: "memory");  // the history buffer is written by reverb_prepare just before us
+        pdl_wait();  // the history buffer is written by reverb_prepare just before us
         if (lane == 0) {
             uint32_t it = 0;
             for (uint32_t si = 0; si < nseg; ++si) {
@@ -231,11 +229,11 @@ __global__ void __launch_bounds__(RV_THREADS, 1) reverb_gemm_kernel(const __grid
                 for (uint32_t i = 0; i < NACC; ++i) __stcg(ws_me + (size_t)i * 256u, acc[i]);
                 __threadfence();  // publish: all 256 consumer threads have stored, then one release store
                 asm volatile("bar.sync 1, 256;" ::: "memory");
-                if (ctid == 0) st_release_u32(a.flags + P, a.epoch);
+                if (ctid == 0) st_release_gpu(a.flags + P, a.epoch);
                 continue;
             }
             if (n_follow) {  // the other slices run in this same wave on CTAs P + 1 ...: they finish when we do
-                for (uint32_t f = lane; f < n_follow; f += 32u) while (ld_acquire_u32(a.flags + P + 1u + f) != a.epoch) { }
+                for (uint32_t f = lane; f < n_follow; f += 32u) while (ld_acquire_gpu(a.flags + P + 1u + f) != a.epoch) { }
                 __syncwarp();
                 for (uint32_t f = 0; f < n_follow; ++f) {  // ascending K: ((first + slice 1) + slice 2) ...
                     const float* wf = a.ws + (size_t)(P + 1u + f) * (RV_BM * RV_BN) + ctid;
@@ -308,19 +306,6 @@ uint32_t reverb_grid_max() {
     return (uint32_t)sms;
 }
 
-// Programmatic dependent launch: every kernel here executes griddepcontrol.wait before it touches its predecessor's results,
-// so the stream-order chain of completions stays intact while launch latency and prologues overlap.
-template <class... KArgs, class... Args>
-static cudaError_t launch_pdl_r(void (*kernel)(KArgs...), dim3 grid, dim3 block, size_t smem, cudaStream_t st, Args&&... args) {
-    cudaLaunchConfig_t cfg{};
-    cfg.gridDim = grid; cfg.blockDim = block; cfg.dynamicSmemBytes = smem; cfg.stream = st;
-    cudaLaunchAttribute attr[1];
-    attr[0].id = cudaLaunchAttributeProgrammaticStreamSerialization;
-    attr[0].val.programmaticStreamSerializationAllowed = 1;
-    cfg.attrs = attr; cfg.numAttrs = 1;
-    return cudaLaunchKernelEx(&cfg, kernel, std::forward<Args>(args)...);
-}
-
 template <uint32_t BN>
 static cudaError_t launch_gemm(const CUtensorMap& tm_a, const CUtensorMap& tm_b, const ReverbGemmArgs& ga, uint32_t grid, cudaStream_t st) {
     static bool attr_set = false;
@@ -329,7 +314,7 @@ static cudaError_t launch_gemm(const CUtensorMap& tm_a, const CUtensorMap& tm_b,
         if (e != cudaSuccess) return e;
         attr_set = true;
     }
-    return launch_pdl_r(reverb_gemm_kernel<BN>, dim3(grid), dim3(RV_THREADS), RV_SMEM_BYTES, st, tm_a, tm_b, ga);
+    return launch_ex(reverb_gemm_kernel<BN>, dim3(grid), dim3(RV_THREADS), RV_SMEM_BYTES, st, true, tm_a, tm_b, ga);
 }
 
 // Tile width for a call: least (waves) x (cycles per k-block) of a paper model (not fitted to per-width timings, and blind to
@@ -353,7 +338,7 @@ cudaError_t launch_reverb(const ReverbCall& rc, cudaStream_t st, std::string* er
     {
         const uint32_t per_block = 256 * 8;
         dim3 grid(rc.C * rc.V, (rc.T + per_block - 1) / per_block < 32 ? (rc.T + per_block - 1) / per_block : 32);
-        cudaError_t e = launch_pdl_r(reverb_prepare, grid, dim3(256), 0, st, rc.in, static_cast<__nv_bfloat16*>(rc.xh), rc.V, rc.C, rc.T, in_pitch, rc.cursor, rc.pitch, rc.zero_first, rc.chan_base);
+        cudaError_t e = launch_ex(reverb_prepare, grid, dim3(256), 0, st, true, rc.in, static_cast<__nv_bfloat16*>(rc.xh), rc.V, rc.C, rc.T, in_pitch, rc.cursor, rc.pitch, rc.zero_first, rc.chan_base);
         if (e != cudaSuccess) return e;
     }
     const uint32_t sms = reverb_grid_max(), tiles_m = (rc.V + RV_BM - 1) / RV_BM;

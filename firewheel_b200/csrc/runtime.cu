@@ -579,7 +579,7 @@ static bool lower_generic(const Schedule& s, const std::vector<int>& sm_of_node,
     const size_t n = s.nodes.size();
     plan->steps.clear(); plan->num_buffers = s.num_buffers;
     if (bus && s.nodes.back().in.size() > (size_t)kMaxBusChannels) { *why = "master bus over more than 8 graph_out channels (FW_MAX_BUS_CHANNELS)"; return false; }
-    uint32_t n_sum_masks = 0;  // nodes whose data-plane body needs the per-block input silence mask
+    uint32_t n_mask_slots = 0;  // nodes whose data-plane body needs the per-block input silence mask
     for (size_t i = 0; i < n; ++i) {
         const SchedNode& sn = s.nodes[i];
         const NodeParams& np = *plan->states[i]->params;
@@ -596,7 +596,7 @@ static bool lower_generic(const Schedule& s, const std::vector<int>& sm_of_node,
         const bool needs_mask = !endpoint && (sp.kind == STEP_CUSTOM || (!sn.out.empty() && (sp.kind == STEP_SUM || (nk.op.mask && !(kind == FW_NODE_VOLUME && sn.in.size() == 2)))));
         if (kind == FW_NODE_CUSTOM && !np.custom->vt.process_device) { *why = std::string("custom node '") + np.custom->debug_name + "' has no process_device: it cannot run on the device (there is no CPU fallback)"; return false; }
         if (needs_mask) {
-            sp.mask_slot = (int)n_sum_masks; plan->nodes[i].mask_slot = ++n_sum_masks;
+            sp.mask_slot = (int)n_mask_slots; plan->nodes[i].mask_slot = ++n_mask_slots;
         }
         if (kind == FW_NODE_DUMMY && !endpoint && !sn.out.empty()) { *why = "a DummyAudioNode inside the graph leaves its outputs stale in the reference (dummy.rs:34-41): not reproducible on the device"; return false; }
         if (kind == FW_NODE_MONO_TO_STEREO && (sn.in.size() != 1 || sn.out.size() != 2)) { *why = "MonoToStereoNode must be 1 -> 2"; return false; }
@@ -616,7 +616,7 @@ static bool lower_generic(const Schedule& s, const std::vector<int>& sm_of_node,
         if (kind == FW_NODE_SAMPLER) sp.sampler_idx = plan->nodes[i].sm1;
         plan->steps.push_back(std::move(sp));
     }
-    plan->rec.n_sum_masks = n_sum_masks;
+    plan->rec.n_mask_slots = n_mask_slots;
     return true;
 }
 
@@ -712,16 +712,15 @@ static bool alloc_plan(const fw_ctx* c, Plan* plan, bool pool, std::string* why)
         r.kt_max = (n_sm ? ramp_blocks : 4u) + 8u * (uint32_t)plan->samplers.size();  // every sample that ends mid-call opens a short transient of its own
         r.kt_max = std::max(2u, std::min(r.kt_max, kc));
     }
-    r.modes = mem.dev<uint32_t>((size_t)r.kt_max * r.n_mode_words * V);
-    r.vals = mem.dev<float>((size_t)r.kt_max * (n_sm ? n_sm : 1) * V);
-    r.curves = mem.dev<float>((size_t)r.kt_max * n_sm * V * F, false);
+    r.modes = mem.dev<uint32_t>(r.modes_count(V));
+    r.vals = mem.dev<float>(r.vals_count(V));
+    r.curves = mem.dev<float>(r.curves_count(V, F), false);
     r.steady_k = mem.dev<uint32_t>(V);
     r.gout_mask = mem.dev<uint64_t>(V);
     r.st_modes = mem.dev<uint32_t>(V);
-    r.st_vals = mem.dev<float>((size_t)(n_sm ? n_sm : 1) * V);
-    const uint32_t n_sum_masks = r.n_sum_masks;
-    r.sum_masks = mem.dev<uint64_t>((size_t)r.kt_max * (n_sum_masks ? n_sum_masks : 1) * V);
-    r.st_sum_masks = mem.dev<uint64_t>((size_t)(n_sum_masks ? n_sum_masks : 1) * V);
+    r.st_vals = mem.dev<float>(r.st_vals_count(V));
+    r.in_masks = mem.dev<uint64_t>(r.in_masks_count(V));
+    r.st_in_masks = mem.dev<uint64_t>(r.st_in_masks_count(V));
     r.error = mem.dev<uint32_t>(1);
     plan->d_bus_mask = mem.dev<uint64_t>(1);
     {   // per-call scratch for one chunk (see Plan)
@@ -735,12 +734,12 @@ static bool alloc_plan(const fw_ctx* c, Plan* plan, bool pool, std::string* why)
             for (const Plan::Operand& o : sp.out) if (o.space == Plan::SCRATCH && !plan->d_tmp[o.index]) plan->d_tmp[o.index] = mem.dev<float>((size_t)V * 2 * Tc, false);
         if (pool) plan->d_pool = mem.dev<float>((size_t)plan->num_buffers * V * Tc, false);
         if (!plan->samplers.empty()) {
-            plan->d_slot_of = mem.dev<uint16_t>((size_t)Kc * V);
+            plan->d_slot_of = mem.dev<uint16_t>(Records::kv_count(Kc, V));
             for (size_t i = 0; i < plan->samplers.size(); ++i) {
-                plan->smp[i].rec = mem.dev<SmpRec>((size_t)Kc * V); plan->smp[i].last_play = mem.dev<uint32_t>(V);
+                plan->smp[i].rec = mem.dev<SmpRec>(Records::kv_count(Kc, V)); plan->smp[i].last_play = mem.dev<uint32_t>(V);
             }
         }
-        for (auto& sp : plan->steps) if (sp.kind == STEP_CUSTOM) { sp.custom_idx = (int)plan->d_custom_masks.size(); plan->d_custom_masks.push_back(mem.dev<uint64_t>((size_t)Kc * V)); }
+        for (auto& sp : plan->steps) if (sp.kind == STEP_CUSTOM) { sp.custom_idx = (int)plan->d_custom_masks.size(); plan->d_custom_masks.push_back(mem.dev<uint64_t>(Records::kv_count(Kc, V))); }
         r.slot_of = plan->d_slot_of;
     }
     {   // the control tables as one image (CtlTables), uploaded once

@@ -12,15 +12,13 @@
 #include <cstdint>
 #include <cstdlib>
 #include <type_traits>
-#include <utility>
 
+#include "device.cuh"
 #include "kernels.cuh"
 #include "plan.hpp"
 
 namespace fw {
 
-__device__ __forceinline__ void t_pdl_launch_dependents() { asm volatile("griddepcontrol.launch_dependents;" ::: "memory"); }
-__device__ __forceinline__ void t_pdl_wait() { asm volatile("griddepcontrol.wait;" ::: "memory"); }
 __device__ __forceinline__ void cp_async16(float4* smem_dst, const float* gsrc) {
     const uint32_t d = (uint32_t)__cvta_generic_to_shared(smem_dst);
     asm volatile("cp.async.cg.shared.global [%0], [%1], 16;" ::"r"(d), "l"(gsrc) : "memory");
@@ -29,6 +27,24 @@ __device__ __forceinline__ void cp_async_commit() { asm volatile("cp.async.commi
 template <int N> __device__ __forceinline__ void cp_async_wait() { asm volatile("cp.async.wait_group %0;" ::"n"(N) : "memory"); }
 
 constexpr int kStateStages = 8;  // state layout [row][8][2] regardless of the cascade length
+
+// One stage of each cascade on input x, in the oracle's op order: returns the stage's output, and its next state in (n1, n2).
+// TDF-II biquad: coefficients {b0, b1, b2, a1, a2}, state {s1, s2}.
+__device__ __forceinline__ float biquad_stage(float b0, float b1, float b2, float a1, float a2, float s1, float s2, float x, float& n1, float& n2) {
+    const float y = __fadd_rn(__fmul_rn(b0, x), s1);
+    n1 = __fadd_rn(__fsub_rn(__fmul_rn(b1, x), __fmul_rn(a1, y)), s2);
+    n2 = __fsub_rn(__fmul_rn(b2, x), __fmul_rn(a2, y));
+    return y;
+}
+// Trapezoidal SVF (include/fw_b200.h): coefficients {a1, a2, a3, m0, m1, m2}, state {ic1, ic2}.
+__device__ __forceinline__ float svf_stage(float a1, float a2, float a3, float m0, float m1, float m2, float ic1, float ic2, float x, float& n1, float& n2) {
+    const float v3 = __fsub_rn(x, ic2);
+    const float v1 = __fadd_rn(__fmul_rn(a1, ic1), __fmul_rn(a2, v3));
+    const float v2 = __fadd_rn(ic2, __fadd_rn(__fmul_rn(a2, ic1), __fmul_rn(a3, v3)));
+    n1 = __fsub_rn(__fmul_rn(2.0f, v1), ic1);
+    n2 = __fsub_rn(__fmul_rn(2.0f, v2), ic2);
+    return __fadd_rn(__fmul_rn(m0, x), __fadd_rn(__fmul_rn(m1, v1), __fmul_rn(m2, v2)));
+}
 
 // Row r of a pass -> its segment (TemporalArgs::seg_rows), the row inside the segment, and its state / ring row.
 struct RowMap { uint32_t seg, rr; size_t srow; };
@@ -69,7 +85,7 @@ __global__ void __launch_bounds__(32) biquad_delay_lanes(TemporalArgs a) {
     static_assert(NS <= L && (L == 1 || L == 2 || L == 4 || L == 8), "lanes per row");
     // No early launch_dependents here: this kernel is issue-bound, and dependents parked at griddepcontrol.wait
     // cost it issue slots. The implicit trigger at exit is enough.
-    t_pdl_wait();  // `in` is produced by the previous kernel of this call
+    pdl_wait();  // `in` is produced by the previous kernel of this call
     const uint32_t lane = threadIdx.x & 31u, s = lane % L;
     const uint32_t row0 = a.row_base + blockIdx.x * ROWS, R = a.R, T = a.T, D = a.D;
     const bool is_first = s == 0, is_last = NS == 0 ? s == 0 : s == (uint32_t)(NS > 0 ? NS - 1 : 0);
@@ -157,18 +173,8 @@ __global__ void __launch_bounds__(32) biquad_delay_lanes(TemporalArgs a) {
         } else {
             const float xi = is_first ? x : q0;
             float n1, n2;
-            if (SVF) {  // (b0, b1, b2, a1, a2, c5) hold (a1, a2, a3, m0, m1, m2); (s1, s2) hold (ic1, ic2)
-                const float v3 = __fsub_rn(xi, s2);
-                const float v1 = __fadd_rn(__fmul_rn(b0, s1), __fmul_rn(b1, v3));
-                const float v2 = __fadd_rn(s2, __fadd_rn(__fmul_rn(b1, s1), __fmul_rn(b2, v3)));
-                n1 = __fsub_rn(__fmul_rn(2.0f, v1), s1);
-                n2 = __fsub_rn(__fmul_rn(2.0f, v2), s2);
-                y = __fadd_rn(__fmul_rn(a1, xi), __fadd_rn(__fmul_rn(a2, v1), __fmul_rn(c5, v2)));
-            } else {
-                y = __fadd_rn(__fmul_rn(b0, xi), s1);
-                n1 = __fadd_rn(__fsub_rn(__fmul_rn(b1, xi), __fmul_rn(a1, y)), s2);
-                n2 = __fsub_rn(__fmul_rn(b2, xi), __fmul_rn(a2, y));
-            }
+            if (SVF) y = svf_stage(b0, b1, b2, a1, a2, c5, s1, s2, xi, n1, n2);  // (b0, b1, b2, a1, a2, c5) hold (a1, a2, a3, m0, m1, m2)
+            else y = biquad_stage(b0, b1, b2, a1, a2, s1, s2, xi, n1, n2);
             if (!CHECK || active) { s1 = n1; s2 = n2; }
             q0 = q1;
             q1 = __shfl_up_sync(0xffffffffu, y, 1);
@@ -232,90 +238,57 @@ __global__ void __launch_bounds__(32) biquad_delay_lanes(TemporalArgs a) {
     }
 }
 
-// Generic path: any T, D, pos. One thread per row, scalar, unskewed. Bit-identical results (same per-stage op order).
-__global__ void __launch_bounds__(64) biquad_delay_generic(TemporalArgs a) {
-    t_pdl_wait();
+// Scalar path: any T, D, pos. One thread per row, unskewed. Bit-identical results (the same stage functions). An SVF pass carries no
+// delay, so the SVF instantiation compiles the delay out. Coefficient rows are 5 floats (biquad) or 6 (SVF).
+template <bool SVF>
+__device__ __forceinline__ void scalar_pass(const TemporalArgs& a) {
+    pdl_wait();
     const uint32_t r = blockIdx.x * blockDim.x + threadIdx.x;
     if (r >= a.R) return;
-    const uint32_t NS = a.ns, T = a.T, D = a.D;
-    float b0[kStateStages], b1[kStateStages], b2[kStateStages], a1[kStateStages], a2[kStateStages], s1[kStateStages], s2[kStateStages];
+    constexpr uint32_t NK = SVF ? 6 : 5;
+    const uint32_t NS = a.ns, T = a.T, D = SVF ? 0u : a.D;
+    float k0[kStateStages], k1[kStateStages], k2[kStateStages], k3[kStateStages], k4[kStateStages], k5[SVF ? kStateStages : 1];
+    float s1[kStateStages], s2[kStateStages];
     const RowMap rm = row_map(a, r);
+    const size_t sr = rm.srow;
     for (uint32_t s = 0; s < NS; ++s) {
-        const float* k = a.coeffs + ((size_t)(rm.rr / a.C) * NS + s) * 5;
-        b0[s] = k[0]; b1[s] = k[1]; b2[s] = k[2]; a1[s] = k[3]; a2[s] = k[4];
-        s1[s] = a.state[(rm.srow * kStateStages + s) * 2]; s2[s] = a.state[(rm.srow * kStateStages + s) * 2 + 1];
+        const float* k = a.coeffs + ((size_t)(rm.rr / a.C) * NS + s) * NK;
+        k0[s] = k[0]; k1[s] = k[1]; k2[s] = k[2]; k3[s] = k[3]; k4[s] = k[4];
+        if (SVF) k5[s] = k[5];
+        s1[s] = a.state[(sr * kStateStages + s) * 2]; s2[s] = a.state[(sr * kStateStages + s) * 2 + 1];
     }
     const float* in = row_in(a, rm);
     float* out = row_out(a, rm);
-    float* ring = D ? a.ring + rm.srow * D : nullptr;
+    float* ring = D ? a.ring + sr * D : nullptr;
     uint32_t p = D ? a.pos % D : 0;
     for (uint32_t n = 0; n < T; ++n) {
         float x = n < a.zero_first ? 0.0f : in[n];
         for (uint32_t s = 0; s < NS; ++s) {
-            const float y = __fadd_rn(__fmul_rn(b0[s], x), s1[s]);
-            s1[s] = __fadd_rn(__fsub_rn(__fmul_rn(b1[s], x), __fmul_rn(a1[s], y)), s2[s]);
-            s2[s] = __fsub_rn(__fmul_rn(b2[s], x), __fmul_rn(a2[s], y));
-            x = y;
+            if (SVF) x = svf_stage(k0[s], k1[s], k2[s], k3[s], k4[s], k5[s], s1[s], s2[s], x, s1[s], s2[s]);
+            else x = biquad_stage(k0[s], k1[s], k2[s], k3[s], k4[s], s1[s], s2[s], x, s1[s], s2[s]);
         }
         if (D) { const float d = ring[p]; ring[p] = x; x = d; p = p + 1 == D ? 0 : p + 1; }
         out[n] = x;
     }
-    for (uint32_t s = 0; s < NS; ++s) { const size_t sr = rm.srow; a.state[(sr * kStateStages + s) * 2] = s1[s]; a.state[(sr * kStateStages + s) * 2 + 1] = s2[s]; }
+    for (uint32_t s = 0; s < NS; ++s) { a.state[(sr * kStateStages + s) * 2] = s1[s]; a.state[(sr * kStateStages + s) * 2 + 1] = s2[s]; }
 }
+// The scalar path's two entry points: their names are the ones profiles and the kernel-coverage test look for.
+__global__ void __launch_bounds__(64) biquad_delay_generic(TemporalArgs a) { scalar_pass<false>(a); }
+__global__ void __launch_bounds__(64) svf_generic(TemporalArgs a) { scalar_pass<true>(a); }
 
-// SVF cascade (spec ours, include/fw_b200.h): one thread per row, scalar. State rows as the biquad's: [row][8][2] = {ic1, ic2}.
-__global__ void __launch_bounds__(64) svf_generic(TemporalArgs a) {
-    t_pdl_wait();
-    const uint32_t r = blockIdx.x * blockDim.x + threadIdx.x;
-    if (r >= a.R) return;
-    const uint32_t NS = a.ns, T = a.T;
-    float a1[kStateStages], a2[kStateStages], a3[kStateStages], m0[kStateStages], m1[kStateStages], m2[kStateStages], ic1[kStateStages], ic2[kStateStages];
-    const RowMap rm = row_map(a, r);
-    const size_t sr = rm.srow;
-    for (uint32_t s = 0; s < NS; ++s) {
-        const float* k = a.coeffs + ((size_t)(rm.rr / a.C) * NS + s) * 6;
-        a1[s] = k[0]; a2[s] = k[1]; a3[s] = k[2]; m0[s] = k[3]; m1[s] = k[4]; m2[s] = k[5];
-        ic1[s] = a.state[(sr * kStateStages + s) * 2]; ic2[s] = a.state[(sr * kStateStages + s) * 2 + 1];
-    }
-    const float* in = row_in(a, rm);
-    float* out = row_out(a, rm);
-    for (uint32_t n = 0; n < T; ++n) {
-        float x = n < a.zero_first ? 0.0f : in[n];
-        for (uint32_t s = 0; s < NS; ++s) {
-            const float v3 = __fsub_rn(x, ic2[s]);
-            const float v1 = __fadd_rn(__fmul_rn(a1[s], ic1[s]), __fmul_rn(a2[s], v3));
-            const float v2 = __fadd_rn(ic2[s], __fadd_rn(__fmul_rn(a2[s], ic1[s]), __fmul_rn(a3[s], v3)));
-            ic1[s] = __fsub_rn(__fmul_rn(2.0f, v1), ic1[s]);
-            ic2[s] = __fsub_rn(__fmul_rn(2.0f, v2), ic2[s]);
-            x = __fadd_rn(__fmul_rn(m0[s], x), __fadd_rn(__fmul_rn(m1[s], v1), __fmul_rn(m2[s], v2)));
-        }
-        out[n] = x;
-    }
-    for (uint32_t s = 0; s < NS; ++s) { a.state[(sr * kStateStages + s) * 2] = ic1[s]; a.state[(sr * kStateStages + s) * 2 + 1] = ic2[s]; }
-}
-
-// Temporal kernels are launched in plain stream order: dependents parked at griddepcontrol.wait compete with an
-// issue-bound kernel.
-template <class... KArgs, class... Args>
-static cudaError_t launch_pdl_t(void (*kernel)(KArgs...), dim3 grid, dim3 block, cudaStream_t st, Args&&... args) {
-    cudaLaunchConfig_t cfg{};
-    cfg.gridDim = grid; cfg.blockDim = block; cfg.dynamicSmemBytes = 0; cfg.stream = st;
-    cfg.attrs = nullptr; cfg.numAttrs = 0;
-    return cudaLaunchKernelEx(&cfg, kernel, std::forward<Args>(args)...);
-}
-
-// Full CTAs + predicated CTAs for the ragged tail.
+// Full CTAs + predicated CTAs for the ragged tail. Temporal kernels are launched without the PDL attribute (pdl = false), in plain
+// stream order: dependents parked at griddepcontrol.wait compete with an issue-bound kernel.
 template <int NS, int L, bool DELAY, bool SVF, int CHF>
 static cudaError_t launch_lanes_c(const TemporalArgs& a, cudaStream_t st) {
     constexpr uint32_t rows1 = 32 / L;
     const uint32_t n_full = a.R / rows1, done = n_full * rows1;
     if (n_full) {
-        cudaError_t e = launch_pdl_t(biquad_delay_lanes<NS, L, DELAY, true, SVF, CHF>, dim3(n_full), dim3(32), st, a);
+        cudaError_t e = launch_ex(biquad_delay_lanes<NS, L, DELAY, true, SVF, CHF>, dim3(n_full), dim3(32), 0, st, false, a);
         if (e != cudaSuccess) return e;
     }
     if (done < a.R) {  // ragged tail
         TemporalArgs t = a; t.row_base = done;
-        return launch_pdl_t(biquad_delay_lanes<NS, L, DELAY, false, SVF, 32>, dim3((a.R - done + rows1 - 1) / rows1), dim3(32), st, t);
+        return launch_ex(biquad_delay_lanes<NS, L, DELAY, false, SVF, 32>, dim3((a.R - done + rows1 - 1) / rows1), dim3(32), 0, st, false, t);
     }
     return cudaSuccess;
 }
@@ -329,7 +302,7 @@ static cudaError_t launch_lanes(const TemporalArgs& a, cudaStream_t st) {
     return launch_lanes_c<NS, L, DELAY, SVF, 32>(a, st);
 }
 
-bool temporal_fast_path(const TemporalArgs& a) {
+static bool temporal_fast_path(const TemporalArgs& a) {
     if (a.T == 0 || a.T % 32u || a.zero_first % 32u) return false;
     if ((reinterpret_cast<uintptr_t>(a.in) | reinterpret_cast<uintptr_t>(a.out) | reinterpret_cast<uintptr_t>(a.ring) | reinterpret_cast<uintptr_t>(a.in2) | reinterpret_cast<uintptr_t>(a.out2)) % 16u) return false;
     if ((a.in_pitch | a.out_pitch) % 4u) return false;
@@ -355,7 +328,7 @@ cudaError_t launch_temporal(const TemporalArgs& a0, cudaStream_t st) {
                 default: return launch_lanes<8, 8, false, true>(a, st);
             }
         }
-        return launch_pdl_t(svf_generic, dim3((a.R + 63) / 64), dim3(64), st, a);
+        return launch_ex(svf_generic, dim3((a.R + 63) / 64), dim3(64), 0, st, false, a);
     }
     if (temporal_fast_path(a)) {
 #define FW_LANES(NS_, L_) (a.D ? launch_lanes<NS_, L_, true>(a, st) : launch_lanes<NS_, L_, false>(a, st))
@@ -372,7 +345,7 @@ cudaError_t launch_temporal(const TemporalArgs& a0, cudaStream_t st) {
         }
 #undef FW_LANES
     }
-    return launch_pdl_t(biquad_delay_generic, dim3((a.R + 63) / 64), dim3(64), st, a);
+    return launch_ex(biquad_delay_generic, dim3((a.R + 63) / 64), dim3(64), 0, st, false, a);
 }
 
 }  // namespace fw
