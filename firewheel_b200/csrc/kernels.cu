@@ -7,7 +7,7 @@
 //   sampler_kernel       K-sampler    SamplerNode: resource fetch + conversion + gain
 //   resampler_*_kernel   K-resampler  polyphase windowed-sinc sample player (+ seek / advance helpers)
 //   combine_kernel       K-combine    radix-16 levels of the bus tree over partial buses
-//   (de)interleave, fill, bus_mask    stream boundary and small helpers
+//   (de)interleave, fill, zero_rows, bus_mask    stream boundary and small helpers
 // temporal.cu holds the biquad / SVF / delay kernels (biquad_delay_lanes; biquad_delay_generic / svf_generic, the scalar path), reverb.cu the wgmma FIR GEMM, exchange.cu the stream hand-over of the master-bus exchange.
 //
 // Bit-exactness rules (SURVEY.md §7 H2): this TU is compiled with --fmad=false, -ftz=false,
@@ -883,6 +883,13 @@ __global__ void fill_kernel(float* __restrict__ p, size_t n, float val) {
     for (size_t i = (size_t)blockIdx.x * blockDim.x + threadIdx.x; i < n; i += (size_t)gridDim.x * blockDim.x) p[i] = val;
 }
 
+// `rows` rows of T frames in each of `groups` groups: row r of group g starts at p + g * group_pitch + r * row_pitch
+__global__ void zero_rows_kernel(float* __restrict__ p, uint32_t T, uint64_t row_pitch, uint32_t groups, uint64_t group_pitch) {
+    const uint32_t t = blockIdx.x * blockDim.x + threadIdx.x;
+    if (t >= T) return;
+    for (uint32_t g = blockIdx.z; g < groups; g += gridDim.z) p[g * group_pitch + blockIdx.y * row_pitch + t] = 0.0f;
+}
+
 // bus mask: V == 1 -> the voice's mask; else ALL(n_out) iff every voice is all-silent (2-port SumNode tree, sum.rs:52-56)
 __global__ void bus_mask_kernel(const uint64_t* __restrict__ gout_mask, uint32_t V, uint32_t n_out, uint64_t* __restrict__ bus_mask) {
     __shared__ int any_audible;
@@ -1011,6 +1018,11 @@ cudaError_t launch_interleave(const float* planar, float* inter, const uint64_t*
 cudaError_t launch_fill(float* p, size_t n, float val, cudaStream_t st) {
     if (n == 0) return cudaSuccess;
     fill_kernel<<<grid_for(n), 256, 0, st>>>(p, n, val);
+    return cudaGetLastError();
+}
+cudaError_t launch_zero_rows(float* p, uint32_t T, uint64_t row_pitch, uint32_t rows, uint32_t groups, uint64_t group_pitch, cudaStream_t st) {
+    if (T == 0 || rows == 0 || groups == 0) return cudaSuccess;
+    zero_rows_kernel<<<dim3((T + 255) / 256, rows, std::min(groups, 65535u)), 256, 0, st>>>(p, T, row_pitch, groups, group_pitch);
     return cudaGetLastError();
 }
 cudaError_t launch_bus_mask(const uint64_t* gout_mask, uint32_t V, uint32_t n_out, uint64_t* bus_mask, cudaStream_t st) {

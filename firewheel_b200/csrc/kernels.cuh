@@ -25,6 +25,8 @@ cudaError_t launch_deinterleave(const float* inter, float* planar, uint32_t V, u
 cudaError_t launch_interleave(const float* planar, float* inter, const uint64_t* masks, uint32_t V, uint32_t C, uint32_t T,
                               uint32_t block_frames, cudaStream_t st);
 cudaError_t launch_fill(float* p, size_t n, float val, cudaStream_t st);
+// +0.0 into `rows` rows of T frames (pitch row_pitch floats) in each of `groups` groups (pitch group_pitch floats) from p
+cudaError_t launch_zero_rows(float* p, uint32_t T, uint64_t row_pitch, uint32_t rows, uint32_t groups, uint64_t group_pitch, cudaStream_t st);
 cudaError_t launch_bus_mask(const uint64_t* gout_mask, uint32_t V, uint32_t n_out, uint64_t* bus_mask, cudaStream_t st);
 cudaError_t launch_bus_signal(uint32_t* word, uint32_t epoch, cudaStream_t st);
 cudaError_t launch_bus_wait(const uint32_t* word, uint32_t epoch, uint32_t* error, uint32_t error_value, cudaStream_t st);

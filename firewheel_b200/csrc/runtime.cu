@@ -278,7 +278,12 @@ struct Plan {
     bool reads_caller_rows = false;  // some node reads the caller's input rows directly (row pitch n_in * frames must fit 32 bits)
     std::vector<std::shared_ptr<NodeDeviceState>> samplers;  // index = CtlTables::smp index
     std::shared_ptr<ResTable> res;  // the context's sample resources, which every sampler and resampler reads (null: the plan has neither)
-    bool bus = false; uint32_t n_sm = 0, c_in = 0, c_out = 0, num_voices = 0, block_frames = 0;
+    // c_in / c_out: graph_in's and graph_out's port counts, which the lowerings use; n_in / n_out: the activated stream's channel counts,
+    // which lay out the caller's rows. Graph_in ports >= n_in read +0.0, stream inputs >= c_in are ignored, caller output rows >= c_out
+    // are written +0.0 and graph_out ports >= n_out are not stored (schedule.rs:213-287, util.rs:96).
+    bool bus = false; uint32_t n_sm = 0, c_in = 0, c_out = 0, n_in = 0, n_out = 0, num_voices = 0, block_frames = 0;
+    uint32_t bus_width() const { return std::min(c_out, n_out); }  // the master bus's live channels; rows from there on are +0.0
+    float* d_zero = nullptr;  // one chunk of +0.0, read with voice stride 0 where the fused chain reads a graph_in port >= n_in
     Records rec{};
     uint64_t* d_bus_mask = nullptr;
     // Per-call scratch, sized on the main thread (lower()) for one chunk of at most `chunk_frames` frames: the stream side
@@ -516,6 +521,7 @@ static bool lower_chain(const Schedule& s, const std::vector<int>& sm_of_node, b
         prev = s.nodes[1].id; first = 2;
     }
     if (width < 1 || width > 2) { *why = "the fused chain supports 1 or 2 channels"; return false; }
+    const uint32_t head_width = first == 1 ? width : 0u;  // graph_in ports the first stage reads from the caller's rows
     auto fed_by_prev = [&](const SchedNode& sn, uint32_t w) {
         if (sn.in.size() != w) return false;
         for (uint32_t p = 0; p < w; ++p) if (sn.in[p].should_clear || sn.in[p].producer != prev || sn.in[p].producer_port != p) return false;
@@ -561,6 +567,12 @@ static bool lower_chain(const Schedule& s, const std::vector<int>& sm_of_node, b
     if (!fed_by_prev(gout, width)) { *why = "graph_out is not fed port-to-port by the end of the chain"; return false; }
     // the last stage must be pointwise when the master bus follows it, and a plan is never empty
     close_pointwise(steps.empty() || (bus && cur.n_ops == 0 && steps.back().kind != STEP_PROG));
+    // Only a pointwise stage addresses the caller's rows channel by channel (a voice stride of n_in / n_out rows, zero rows for graph_in
+    // ports >= n_in, graph_out ports >= n_out left out); a temporal or sampler stage reads and writes [V][C] rows.
+    if ((head_width && head_width != plan->n_in && steps.front().kind != STEP_PROG) ||
+        (!bus && width != plan->n_out && steps.back().kind != STEP_PROG)) {
+        *why = "a stateful stage at the end of the chain on a stream whose channel counts differ from the graph's ports"; return false;
+    }
     for (uint32_t si = 0; si < steps.size(); ++si) {
         const bool last = si + 1 == steps.size();
         for (Plan::Operand& o : steps[si].in) o = si == 0 ? Plan::Operand{Plan::CALLER_IN, 0, o.C} : Plan::Operand{Plan::SCRATCH, (si - 1) & 1, o.C};
@@ -578,7 +590,7 @@ static_assert(kMaxBusChannels == FW_MAX_BUS_CHANNELS, "plan.hpp and the C header
 static bool lower_generic(const Schedule& s, const std::vector<int>& sm_of_node, bool bus, Plan* plan, std::string* why) {
     const size_t n = s.nodes.size();
     plan->steps.clear(); plan->num_buffers = s.num_buffers;
-    if (bus && s.nodes.back().in.size() > (size_t)kMaxBusChannels) { *why = "master bus over more than 8 graph_out channels (FW_MAX_BUS_CHANNELS)"; return false; }
+    if (bus && plan->bus_width() > (uint32_t)kMaxBusChannels) { *why = "master bus over more than 8 graph_out channels (FW_MAX_BUS_CHANNELS)"; return false; }
     uint32_t n_mask_slots = 0;  // nodes whose data-plane body needs the per-block input silence mask
     for (size_t i = 0; i < n; ++i) {
         const SchedNode& sn = s.nodes[i];
@@ -588,8 +600,11 @@ static bool lower_generic(const Schedule& s, const std::vector<int>& sm_of_node,
         Plan::Step sp; sp.node = plan->states[i]; sp.sm0 = sm_of_node[i];
         for (const InAssign& a : sn.in) { sp.in.push_back(Plan::Operand{Plan::POOL, a.buffer, 1}); if (a.should_clear) sp.clear.push_back(a.buffer); }
         for (const OutAssign& a : sn.out) sp.out.push_back(Plan::Operand{Plan::POOL, a.buffer, 1});
-        if (i == 0) for (uint32_t p = 0; p < sn.out.size(); ++p) sp.in.push_back(Plan::Operand{Plan::CALLER_IN, p, 1});
-        if (i + 1 == n && !bus) for (uint32_t p = 0; p < sn.in.size(); ++p) sp.out.push_back(Plan::Operand{Plan::CALLER_OUT, p, 1});
+        // graph_in copies the stream's channels and clears its ports >= n_in; graph_out stores its ports < n_out (schedule.rs:244-252,269)
+        if (i == 0) for (uint32_t p = 0; p < sn.out.size(); ++p) {
+            if (p < plan->n_in) sp.in.push_back(Plan::Operand{Plan::CALLER_IN, p, 1}); else sp.clear.push_back(sn.out[p].buffer);
+        }
+        if (i + 1 == n && !bus) for (uint32_t p = 0; p < sn.in.size() && p < plan->n_out; ++p) sp.out.push_back(Plan::Operand{Plan::CALLER_OUT, p, 1});
         const NodeKind& nk = node_kind(kind);
         sp.kind = kind == FW_NODE_SUM && sn.in.size() == sn.out.size() ? STEP_PROG : nk.step;  // a 1-port SumNode is a copy (sum.rs:58-65)
         // bodies that branch on the input silence mask (see silence_fix_kernel / sum_kernel)
@@ -660,7 +675,7 @@ static void fuse_generic(const Schedule& s, Plan* plan) {
     for (size_t i = 1; i + 1 < n; ++i) {
         if (!(stereo_pointwise(i) || (nk(i).step == STEP_TEMPORAL && connected(i) && !s.nodes[i].in.empty()))) continue;
         bool all = true;
-        for (const InAssign& a : s.nodes[i].in) if (a.producer != s.nodes[0].id || a.producer_port >= alias_cons.size()) all = false;
+        for (const InAssign& a : s.nodes[i].in) if (a.producer != s.nodes[0].id || a.producer_port >= alias_cons.size() || a.producer_port >= plan->n_in) all = false;
         if (!all) continue;
         for (size_t k = 0; k < s.nodes[i].in.size(); ++k) {
             const uint32_t port = s.nodes[i].in[k].producer_port;
@@ -726,13 +741,14 @@ static bool alloc_plan(const fw_ctx* c, Plan* plan, bool pool, std::string* why)
     {   // per-call scratch for one chunk (see Plan)
         const uint32_t Tc = c->max_call_frames, Kc = (Tc + F - 1) / F;
         plan->chunk_frames = Tc; plan->chunk_blocks = Kc;
-        const uint32_t n_out = plan->c_out, groups = chain_voice_groups(V);
+        const uint32_t n_out = plan->bus_width(), groups = chain_voice_groups(V);
         if (plan->bus) {
             plan->d_part[0] = mem.dev<float>((size_t)groups * n_out * Tc, false); plan->d_part[1] = mem.dev<float>((size_t)((groups + 15) / 16) * n_out * Tc, false);
         }
         for (const Plan::Step& sp : plan->steps)
             for (const Plan::Operand& o : sp.out) if (o.space == Plan::SCRATCH && !plan->d_tmp[o.index]) plan->d_tmp[o.index] = mem.dev<float>((size_t)V * 2 * Tc, false);
         if (pool) plan->d_pool = mem.dev<float>((size_t)plan->num_buffers * V * Tc, false);
+        else if (plan->n_in < plan->c_in) plan->d_zero = mem.dev<float>(Tc);
         if (!plan->samplers.empty()) {
             plan->d_slot_of = mem.dev<uint16_t>(Records::kv_count(Kc, V));
             for (size_t i = 0; i < plan->samplers.size(); ++i) {
@@ -766,9 +782,7 @@ static bool lower(fw_ctx* c, const Schedule& s, Plan* plan, std::string* why) {
     if (!lower_control(c, s, plan, &sm_of_node, why)) return false;
     const SchedNode& gin = s.nodes.front();
     const SchedNode& gout = s.nodes.back();
-    if (gin.out.size() != c->n_in) { *why = "stream input channels must equal the graph_in port count on the device path"; return false; }
-    if (gout.in.size() != c->n_out) { *why = "stream output channels must equal the graph_out port count on the device path"; return false; }
-    plan->c_in = (uint32_t)gin.out.size(); plan->c_out = (uint32_t)gout.in.size();
+    plan->c_in = (uint32_t)gin.out.size(); plan->c_out = (uint32_t)gout.in.size(); plan->n_in = c->n_in; plan->n_out = c->n_out;
     const bool bus = c->cfg.master_bus != 0;
     const bool chain = lower_chain(s, sm_of_node, bus, plan, why);
     if (!chain) {
@@ -1679,33 +1693,50 @@ static int enqueue_chunk(fw_processor* p, Plan& pl, const float* d_in, float* d_
     // ---- data plane: the steps in order (see Plan::Step); the generic lowering's pool buffer reuse is the reference's
     // (compiler.rs:302-412): it is valid for any execution that respects the schedule order, and each step finishes all blocks of the
     // chunk before the next one starts ----
-    if (pl.reads_caller_rows && (uint64_t)pl.c_in * ck.Tfull > 0xffffffffull) { g_dev_err = "input rows of more than 2^32 / channels frames"; return FW_PROC_BAD_ARGS; }
+    if (pl.reads_caller_rows && (uint64_t)pl.n_in * ck.Tfull > 0xffffffffull) { g_dev_err = "input rows of more than 2^32 / channels frames"; return FW_PROC_BAD_ARGS; }
     auto out_rows = [&](const Plan::Operand& o) -> float* {
         return o.space == Plan::CALLER_OUT ? d_out + ck.t0 + (size_t)o.index * ck.Tfull : o.space == Plan::POOL ? pl.d_pool + (size_t)o.index * V * T : pl.d_tmp[o.index];
     };
     auto in_rows = [&](const Plan::Operand& o) -> const float* { return o.space == Plan::CALLER_IN ? d_in + ck.t0 + (size_t)o.index * ck.Tfull : out_rows(o); };
-    auto pitch = [&](const Plan::Operand& o) -> uint64_t {
-        if (o.space == Plan::POOL || o.space == Plan::SCRATCH) return T;
-        return o.C > 1 ? ck.Tfull : (uint64_t)(o.space == Plan::CALLER_IN ? pl.c_in : pl.c_out) * ck.Tfull;
+    // floats between the channels of one operand, and between its voices: the caller's rows hold n_in / n_out channels per voice
+    auto vstride = [&](const Plan::Operand& o) -> uint64_t {
+        if (o.space == Plan::POOL || o.space == Plan::SCRATCH) return (uint64_t)o.C * T;
+        return (uint64_t)(o.space == Plan::CALLER_IN ? pl.n_in : pl.n_out) * ck.Tfull;
     };
+    auto pitch = [&](const Plan::Operand& o) -> uint64_t { return o.space == Plan::POOL || o.space == Plan::SCRATCH ? T : o.C > 1 ? ck.Tfull : vstride(o); };
     RowBlock rows[64];                   // rows[k]: input operand k and output operand k
     const float* in[64]; float* out[64];  // every input and output channel
     for (size_t si = 0; si < pl.steps.size(); ++si) {
         const Plan::Step& sp = pl.steps[si];
         const uint32_t nb = (uint32_t)std::max(sp.in.size(), sp.out.size());
         uint32_t ni = 0, no = 0; uint64_t ivs = 0, ovs = 0;  // channels and voice strides
+        uint32_t ni_real = 0;  // in[ni_real..ni) are graph_in ports >= n_in: d_zero (only the fused chain's first stage has them)
         in[0] = in[1] = nullptr; out[0] = out[1] = nullptr;  // chain_args reads prog.c_in slots; the generic bus step has no outputs
         for (uint32_t k = 0; k < nb; ++k) rows[k] = RowBlock{};
         for (uint32_t k = 0; k < sp.in.size(); ++k) {
+            const Plan::Operand& o = sp.in[k];
             RowBlock& r = rows[k];
-            r.in = in_rows(sp.in[k]); r.in_pitch = pitch(sp.in[k]); r.C = sp.in[k].C; ivs = r.C * r.in_pitch;
-            for (uint32_t c = 0; c < r.C; ++c) in[ni++] = r.in + c * r.in_pitch;
+            r.in = in_rows(o); r.in_pitch = pitch(o); r.C = o.C; ivs = vstride(o);
+            for (uint32_t c = 0; c < r.C; ++c) {
+                const bool zero = o.space == Plan::CALLER_IN && o.index + c >= pl.n_in;
+                in[ni++] = zero ? pl.d_zero : r.in + c * r.in_pitch;
+                if (!zero) ni_real = ni;
+            }
         }
         for (uint32_t k = 0; k < sp.out.size(); ++k) {
+            const Plan::Operand& o = sp.out[k];
             RowBlock& r = rows[k];
-            r.out = out_rows(sp.out[k]); r.out_pitch = pitch(sp.out[k]); r.C = sp.out[k].C; ovs = r.C * r.out_pitch;
-            for (uint32_t c = 0; c < r.C; ++c) out[no++] = r.out + c * r.out_pitch;
+            r.out = out_rows(o); r.out_pitch = pitch(o); r.C = o.C; ovs = vstride(o);
+            for (uint32_t c = 0; c < r.C && (o.space != Plan::CALLER_OUT || o.index + c < pl.n_out); ++c) out[no++] = r.out + c * r.out_pitch;
         }
+        // Voice stride of a chain launch from input channel c. Graph_in ports >= n_in (the fused chain's first stage): a second channel is
+        // read as +0.0 by the one-channel variant, a launch with no real channel reads the zero row for every voice.
+        auto in_stride = [&](ChainProgram& pr, uint32_t c) -> uint64_t {
+            if (ni_real == ni) return ivs;
+            if (c >= ni_real) return 0;
+            if (c + 1 == ni_real && pr.c_in > 1) pr.c_in = 1;
+            return ivs;
+        };
         const bool caller = !sp.in.empty() && sp.in[0].space == Plan::CALLER_IN;  // Q11 applies to the caller's rows only
         const uint32_t zf = caller ? ck.zero_first : 0u;
         for (uint32_t b : sp.clear) { if (!FW_CUDA(launch_fill(pl.d_pool + (size_t)b * V * T, (size_t)V * T, 0.0f, p->stream))) return FW_PROC_DEVICE_ERROR; p->launches++; }
@@ -1716,14 +1747,25 @@ static int enqueue_chunk(fw_processor* p, Plan& pl, const float* d_in, float* d_
             case STEP_REVERB: rc = run_reverb(p, *sp.node, rows, nb, T, zf); break;
             case STEP_PROG:
                 if (pl.bus && si + 1 == pl.steps.size()) {
-                    ChainArgs xa = chain_args(pl, ck, sp.prog, in, ivs, out, ovs, caller);
-                    rc = run_bus_stage(p, pl, xa, pl.c_out, ck, d_out + ck.t0);
+                    ChainProgram pr = sp.prog;
+                    const uint32_t live = pl.bus_width();
+                    if (live < pl.c_out) {  // graph_out ports >= n_out do not reach the bus
+                        if (live == 0) break;
+                        if (pr.c_in > 2) pr.c_in = live;  // graph_out's copy reads only the live channels
+                        pr.c_out = std::min(pr.c_out, live);
+                    }
+                    const uint64_t vs = in_stride(pr, 0);
+                    ChainArgs xa = chain_args(pl, ck, pr, in, vs, out, ovs, caller);
+                    rc = run_bus_stage(p, pl, xa, live, ck, d_out + ck.t0);
                     break;
                 }
                 for (uint32_t c = 0, nc = std::min(ni, no); c < (sp.pairs ? nc : 1u); c += 2) {
                     ChainProgram pr = sp.prog;
                     if (sp.pairs && c + 1 == nc) pr.c_in = pr.c_out = 1;
-                    if (!FW_LAUNCH(p, 1, 1, launch_chain(chain_args(pl, ck, pr, in + c, ivs, out + c, ovs, caller), false, p->stream))) return FW_PROC_DEVICE_ERROR;
+                    pr.c_out = std::min(pr.c_out, no - c);  // graph_out ports >= n_out are not stored
+                    if (pr.c_out == 0) continue;
+                    const uint64_t vs = in_stride(pr, c);
+                    if (!FW_LAUNCH(p, 1, 1, launch_chain(chain_args(pl, ck, pr, in + c, vs, out + c, ovs, caller), false, p->stream))) return FW_PROC_DEVICE_ERROR;
                 }
                 for (uint32_t c = 0; sp.mask_slot >= 0 && c < no; ++c) {  // test: the inputs output c is made of
                     SilenceFixArgs fa{};
@@ -1769,6 +1811,10 @@ static int enqueue_chunk(fw_processor* p, Plan& pl, const float* d_in, float* d_
             }
         }
         if (rc != FW_PROC_OK) return rc;
+    }
+    if (pl.n_out > pl.c_out) {  // caller output rows >= c_out, per voice or on the bus, are +0.0 (util.rs:96)
+        const uint32_t groups = pl.bus ? 1u : V;
+        if (!FW_LAUNCH(p, 1, 1, launch_zero_rows(d_out + ck.t0 + (size_t)pl.c_out * ck.Tfull, T, ck.Tfull, pl.n_out - pl.c_out, groups, (uint64_t)pl.n_out * ck.Tfull, p->stream))) return FW_PROC_DEVICE_ERROR;
     }
     return FW_PROC_OK;
 }
@@ -1826,6 +1872,7 @@ static int run_chunk(fw_processor* p, Plan& pl, const float* d_in, float* d_out,
 static int proc_call(fw_processor* p, const float* d_in, float* d_out, uint32_t n_in, uint32_t n_out, uint64_t frames64) {
     if (frames64 > 0x7fffffffull) return FW_PROC_BAD_ARGS;
     const uint32_t T = (uint32_t)frames64, V = p->num_voices;
+    if (n_in != p->n_in || n_out != p->n_out) { g_dev_err = "channel counts do not match the activated stream"; return FW_PROC_BAD_ARGS; }
     const size_t out_rows = (size_t)(p->bus ? 1 : V) * n_out;
     cudaSetDevice(p->device);
     // zero frames [t0, T) of every output row
@@ -1860,7 +1907,6 @@ static int proc_call(fw_processor* p, const float* d_in, float* d_out, uint32_t 
         proc_poll(p);                                                                        // process_block :214
         if (!p->running) { silence_from(b * F); rc = FW_PROC_DROP_PROCESSOR; break; }        // :150-155
         Plan& pl = *p->plan;
-        if (n_in != pl.c_in || n_out != pl.c_out) { g_dev_err = "channel counts do not match the compiled graph"; return FW_PROC_BAD_ARGS; }
         while (next_cmd < p->pend_n && p->pend[next_cmd].block < b) ++next_cmd;
         const bool have_cmds = next_cmd < p->pend_n && p->pend[next_cmd].block == b;
         if (have_cmds || !pl.samplers.empty()) { if (!apply_commands(p, pl, b)) return FW_PROC_DEVICE_ERROR; }
@@ -1886,9 +1932,11 @@ static int proc_call(fw_processor* p, const float* d_in, float* d_out, uint32_t 
     return rc;
 }
 
+// The graph_out mask covers the stream's n_out channels (schedule.rs:269); channels >= graph_out's ports are never flagged, so with
+// more than one voice a bus with such channels is never all silent (the tree's SumNodes, sum.rs:52-56).
 static uint64_t bus_mask_from(const uint64_t* masks, uint32_t V, uint32_t n_out) {
-    if (V == 1) return masks[0];
     const uint64_t all = n_out >= 64 ? ~0ull : ((1ull << n_out) - 1ull);
+    if (V == 1) return masks[0] & all;
     for (uint32_t v = 0; v < V; ++v) if ((masks[v] & all) != all) return 0;
     return all;
 }
@@ -1943,7 +1991,7 @@ static int host_call(fw_processor* p, uint32_t n_in, uint32_t n_out, uint64_t fr
     if (!FW_CUDA(cudaStreamSynchronize(p->stream))) return FW_PROC_DEVICE_ERROR;
     if (ran) {
         if (check_device_error(p, since_epoch)) return FW_PROC_DEVICE_ERROR;
-        if (out_mask) *out_mask = p->bus ? bus_mask_from(p->h_masks, V, n_out) : p->h_masks[0];
+        if (out_mask) *out_mask = p->bus ? bus_mask_from(p->h_masks, V, n_out) : p->h_masks[0] & (n_out >= 64 ? ~0ull : (1ull << n_out) - 1ull);
     }
     return rc;
 }

@@ -199,9 +199,8 @@ enum fw_compile_error {
     FW_COMPILE_MESSAGE_CHANNEL_FULL = 7,
     /* product only: the graph is valid for the reference but has no device lowering yet. The refusals: a user node without
      * process_device; a DummyAudioNode with outputs inside the graph; a MonoToStereoNode that is not 1 -> 2 or a StereoToMonoNode that
-     * is not 2 -> 1; a master bus over more than FW_MAX_BUS_CHANNELS graph_out channels; stream channel counts other than graph_in's /
-     * graph_out's port counts; silence flags of one voice that do not fit in one SM's shared memory (about 930 000 pool buffers on an
-     * H100). The number of nodes, buffers, ports, smoothed parameters, samplers and resamplers is not limited otherwise. */
+     * is not 2 -> 1; a master bus over more than FW_MAX_BUS_CHANNELS live channels (graph_out ports that are also stream channels);
+     * silence flags of one voice that do not fit in one SM's shared memory (about 930 000 pool buffers on an H100). The number of nodes, buffers, ports, smoothed parameters, samplers and resamplers is not limited otherwise. */
     FW_COMPILE_UNSUPPORTED_ON_DEVICE = 100
 };
 /* FirewheelProcessorStatus (processor.rs:12-16) + device-error code */
@@ -385,6 +384,16 @@ FW_EXPORT int FW_FN(ctx_update)(fw_ctx* ctx, fw_update_status* out);            
 FW_EXPORT void* FW_FN(ctx_deactivate)(fw_ctx* ctx, int stream_is_running);          /* context.rs:162 */
 
 /* ---- the hot path (processor.rs:61-248, schedule.rs:213-343) ---------------------------- */
+/* num_in_channels / num_out_channels must equal the counts given to ctx_activate; they may differ from graph_in's port count G_in
+ * and graph_out's port count G_out, as in the reference (schedule.rs:213-287, util.rs:44-147):
+ *   S1 n_in < G_in:   graph_in ports >= n_in read +0.0 in every block; downstream they are live zeros, not silent (graph_in's
+ *                     Dummy overwrites their flags, schedule.rs:338-341);
+ *   S2 n_in > G_in:   input channels >= G_in are ignored;
+ *   S3 n_out > G_out: output channels >= G_out are written +0.0 and never flagged in a silence mask; with the master bus and two or
+ *                     more voices the bus's SumNodes then never see all inputs flagged, so the bus mask is 0 (sum.rs:52-56);
+ *   S4 n_out < G_out: graph_out ports >= n_out are not read; silence masks cover the n_out channels.
+ * The master bus mixes min(G_out, n_out) channels. process_interleaved interleaves a stereo pair as one (util.rs:123-147) only when
+ * n_out == 2 and G_out >= 2 (processor.rs:122-133). */
 FW_EXPORT int FW_FN(processor_process_interleaved)(fw_processor* p, const float* input, float* output,
                                                    uint32_t num_in_channels, uint32_t num_out_channels,
                                                    uint64_t frames, double stream_time_secs,
@@ -403,7 +412,8 @@ FW_EXPORT void FW_FN(processor_free)(fw_processor* p);                          
 /* ---- pull-style stream backend (product only; replaces firewheel-cpal's DataCallback, crates/firewheel-cpal/src/lib.rs:378-449)
  * cpal calls the processor from its device callback; here a producer thread renders `period_frames` at a time, ahead of
  * the consumer, into a host ring of `ring_periods` periods, and the consumer PULLS interleaved frames. Like cpal (lib.rs:177)
- * the stream has no input channels. stream_time_secs handed to the graph is the sample clock (frames rendered / sample
+ * the stream has no input channels: activate with num_in_channels = 0, and graph_in's ports read +0.0 (S1 above); a graph whose
+ * graph_out has fewer ports than the device has channels plays on the first ones (S3). stream_time_secs handed to the graph is the sample clock (frames rendered / sample
  * rate). A pull that finds the ring empty zero-fills the rest, reports FW_STREAM_OUTPUT_UNDERFLOW, and the next rendered
  * period carries that flag in its stream_status (lib.rs:424-428). After DropProcessor pulls deliver silence (lib.rs:446-448).
  * Requires one output stream per context: num_voices == 1 or master_bus == 1. While a stream is open the processor must not
